@@ -428,8 +428,9 @@ int in_place_host(float *buf, size_t bytes, Op op) {
 
 extern "C" {
 
-// Test / developer hook: the switches above (initialised from the MB200_* environment variables of the same upper-case
-// names) can be flipped at run time, e.g. to compare a specialised kernel with the generic one in one process.
+// Test / developer hook: the switches above and the tuning knobs of runtime.cu (initialised from the MB200_* environment
+// variables of the same upper-case names) can be changed at run time, e.g. to compare a specialised kernel with the
+// generic one in one process.  mb200_get_option also reads the per-family launch counters.
 int mb200_set_option(const char *name, int value) {
   if (!name) return fail(MB200_EINVAL, "set_option: null name");
   Knobs &k = knobs();
@@ -442,7 +443,11 @@ int mb200_set_option(const char *name, int value) {
   else if (n == "no_fused_unsharp") k.no_fused_unsharp = v;
   else if (n == "resize_fused") k.resize_fused = v;
   else if (n == "conv_mma") set_conv_mma(value);
-  else return fail(MB200_EINVAL, "set_option: unknown option '%s'", name);
+  else {
+    const int rc = set_tuning_knob(name, value);
+    if (rc == MB200_EINVAL) return fail(MB200_EINVAL, "set_option: %d is not a valid value of '%s'", value, name);
+    if (rc != MB200_OK) return fail(MB200_EINVAL, "set_option: unknown option '%s'", name);
+  }
   return MB200_OK;
 }
 
@@ -458,7 +463,8 @@ int mb200_get_option(const char *name, int *value) {
   else if (n == "resize_fused") *value = k.resize_fused;
   else if (n == "conv_mma") *value = conv_mma_enabled();
   else if (n == "conv_mma_launches") *value = static_cast<int>(conv_mma_launches() & 0x7fffffff);
-  else return fail(MB200_EINVAL, "get_option: unknown option '%s'", name);
+  else if (!get_tuning_knob(name, value) && !get_family_count(name, value))
+    return fail(MB200_EINVAL, "get_option: unknown option '%s'", name);
   return MB200_OK;
 }
 
@@ -575,6 +581,21 @@ int mb200_resize_image_ex_dev(const float *src, size_t width, size_t height, int
   if (out_width == width && out_height == height && filter == MB200_UndefinedFilter) {            // :3793-3795
     cudaError_t e = cudaMemcpyAsync(dst, src, width * height * px, cudaMemcpyDeviceToDevice, s);
     return e == cudaSuccess ? MB200_OK : cuda_fail(e, "resize: clone");
+  }
+  if (((reinterpret_cast<uintptr_t>(src) | reinterpret_cast<uintptr_t>(dst)) & 15) != 0) {
+    // The resize kernels move whole pixels (float2 / float4 loads and stores, 16-byte cp.async and TMA copies): a pixel
+    // cache that is not 16-byte aligned (a view that starts inside a buffer) is resized through aligned copies.
+    StreamAlloc in(s), out(s);
+    rc = in.alloc(width * height * px);
+    if (!rc) rc = out.alloc(out_width * out_height * px);
+    if (rc) return rc;
+    cudaError_t e = cudaMemcpyAsync(in.ptr, src, width * height * px, cudaMemcpyDeviceToDevice, s);
+    if (e != cudaSuccess) return cuda_fail(e, "resize: aligned copy of the source");
+    rc = mb200_resize_image_ex_dev(static_cast<const float *>(in.ptr), width, height, channels,
+                                   static_cast<float *>(out.ptr), out_width, out_height, filter, options, s);
+    if (rc) return rc;
+    e = cudaMemcpyAsync(dst, out.ptr, out_width * out_height * px, cudaMemcpyDeviceToDevice, s);
+    return e == cudaSuccess ? MB200_OK : cuda_fail(e, "resize: result copy");
   }
   auto reciprocal = [](double x) { return std::fabs(x) >= 1.0e-12 ? 1.0 / x : (x < 0 ? -1.0e12 : 1.0e12); };
   const double x_factor = static_cast<double>(out_width) * reciprocal(static_cast<double>(width));

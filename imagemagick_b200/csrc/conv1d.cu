@@ -180,8 +180,9 @@ __global__ void __launch_bounds__(128, MINB) conv_row_kernel(const Conv1dArgs a,
   const int total = a.strip + NT - 1;
   const int wmax = a.width - 1, hmax = a.height - 1;
 
-  // ---- stage the tile: rows_per_cta x total source pixels, x edge-clamped
-  if (ch == 4) {
+  // ---- stage the tile: rows_per_cta x total source pixels, x edge-clamped (whole pixels when they are 16-byte aligned;
+  // the matrix and pair kernels decline unaligned sources and leave them to this kernel)
+  if (ch == 4 && (reinterpret_cast<uintptr_t>(a.src) & 15) == 0) {
     const int n = rows_per_cta * total;
     for (int idx = threadIdx.x; idx < n; idx += 128) {
       const int r = idx / total, px = idx - r * total;
@@ -646,35 +647,16 @@ __global__ void __launch_bounds__(128, MINB) conv_pair_async_kernel(const Conv1d
   asm volatile("cp.async.wait_group 0;" );
 }
 
-// Developer tuning knobs: environment variables read ONCE per process (defaults are the measured best).
-struct Tuning {
-  int pair, pair_async, pair_async_col, col_rot, row_pair_rot, row_rot;
-  Tuning() {
-    auto get = [](const char *name, int fallback) {
-      const char *v = getenv(name);
-      return (v && *v) ? atoi(v) : fallback;
-    };
-    pair = get("MB200_PAIR", 1);
-    pair_async = get("MB200_PAIR_ASYNC", 1);
-    pair_async_col = get("MB200_PAIR_ASYNC_COL", -1);     // -1: cp.async ring for windows shorter than 33 taps
-    col_rot = get("MB200_COL_ROT", 16);
-    row_pair_rot = get("MB200_ROW_PAIR_ROT", 16);
-    row_rot = get("MB200_ROW_ROT", 0);
-    // (3 CTAs per SM for the NT = 33 cp.async kernels -- __launch_bounds__(128, 3), 168 registers, spills -- were slower
-    //  than 2: the third warp per scheduler does not pay for the spilled accumulators.)
-  }
-};
-const Tuning &tuning() {
-  static const Tuning t;
-  return t;
-}
-
-// The RGBA pair kernels of one pass.  PADDED / EPI select the instantiation; everything else is the r01 choice.
+// The RGBA pair kernels of one pass.  PADDED / EPI select the instantiation; everything else is the r01 choice.  Returns
+// the family of the kernel it launched, or kLaunchFamilies when the grid does not fit (nothing launched).
+// (3 CTAs per SM for the NT = 33 cp.async kernels -- __launch_bounds__(128, 3), 168 registers, spills -- were slower than
+//  2: the third warp per scheduler does not pay for the spilled accumulators.)
 template <int NT, bool PADDED>
-void launch_pair(const Conv1dArgs &a, const Taps<NT> &taps, int axis, int io, bool fuse_unsharp, cudaStream_t stream) {
-  const Tuning &t = tuning();
+LaunchFamily launch_pair(const Conv1dArgs &a, const Taps<NT> &taps, int axis, int io, bool fuse_unsharp,
+                         const TuningKnobs &t, cudaStream_t stream) {
   if (axis == 1) {
     dim3 grid((a.rc / 2 + 127) / 128, (a.height + a.strip - 1) / a.strip);
+    if (grid.y > 65535) return kLaunchFamilies;
     // NT = 33 is FP64-bound: the register-ring kernel (+ L2 prefetch) wins; shorter windows are closer to
     // the HBM roof and gain from the cp.async ring (sigma=2: 1.36 -> 1.22 ms for the whole blur).
     const bool async = (t.pair_async_col < 0 ? NT < 33 : t.pair_async_col != 0) && t.pair_async != 0;
@@ -685,14 +667,17 @@ void launch_pair(const Conv1dArgs &a, const Taps<NT> &taps, int axis, int io, bo
     else if (fuse_unsharp) conv_pair_kernel<NT, 2, 1, 0, NT == 33, PADDED, 1><<<grid, 128, 0, stream>>>(a, taps);
     else if (async) conv_pair_async_kernel<NT, 2, 1, 0, PADDED><<<grid, 128, 0, stream>>>(a, taps);
     else conv_pair_kernel<NT, 2, 1, 0, NT == 33, PADDED><<<grid, 128, 0, stream>>>(a, taps);
+    return async && io != 2 ? kConvPairAsync : kConvPair;
   } else {
     dim3 grid((a.width + a.strip - 1) / a.strip, (a.height + 63) / 64);
+    if (grid.y > 65535) return kLaunchFamilies;
     const bool async = t.pair_async != 0;
     if (io == 1 && async) conv_pair_async_kernel<NT, 2, 0, 1, PADDED><<<grid, 128, 0, stream>>>(a, taps);
     else if (io == 1) conv_pair_kernel<NT, 2, 0, 1, false, PADDED><<<grid, 128, 0, stream>>>(a, taps);
     else if (io == 2) conv_pair_kernel<NT, 2, 0, 2, false, PADDED><<<grid, 128, 0, stream>>>(a, taps);
     else if (async) conv_pair_async_kernel<NT, 2, 0, 0, PADDED><<<grid, 128, 0, stream>>>(a, taps);
     else conv_pair_kernel<NT, 2, 0, 0, false, PADDED><<<grid, 128, 0, stream>>>(a, taps);
+    return async && io != 2 ? kConvPairAsync : kConvPair;
   }
 }
 
@@ -703,7 +688,7 @@ int launch_nt(const Conv1dArgs &base, int axis, const double *taps_host, int nta
   for (int i = 0; i < NT; ++i) taps.k[i] = i < ntaps ? taps_host[i] : 0.0;   // zero padding past the window
   Conv1dArgs a = base;
   a.ntaps = ntaps;
-  const Tuning &t = tuning();
+  const TuningKnobs t = tuning_knobs();
   if (io != 0 && !(MODE == 4 && NT <= 33)) return MB200_EUNSUPPORTED;
   const bool pair_ok = MODE == 4 && a.bias == 0.0 && NT <= 33 && (io != 0 || t.pair != 0) &&
                        ((reinterpret_cast<uintptr_t>(a.src) | reinterpret_cast<uintptr_t>(a.dst)) & 15) == 0;
@@ -716,8 +701,10 @@ int launch_nt(const Conv1dArgs &base, int axis, const double *taps_host, int nta
       a.strip = (axis == 1 ? t.col_rot : t.row_pair_rot) * NT + 1;
       a.seg_w = 16;                                  // rows of L2 prefetch ahead of the register ring (L2PF kernels)
       const bool fuse = axis == 1 && io == 0 && a.aux != nullptr && (reinterpret_cast<uintptr_t>(a.aux) & 15) == 0;
-      if (ntaps != NT) launch_pair<NT, true>(a, taps, axis, io, fuse, stream);
-      else launch_pair<NT, false>(a, taps, axis, io, fuse, stream);
+      const LaunchFamily family = ntaps != NT ? launch_pair<NT, true>(a, taps, axis, io, fuse, t, stream)
+                                              : launch_pair<NT, false>(a, taps, axis, io, fuse, t, stream);
+      if (family == kLaunchFamilies) return MB200_EUNSUPPORTED;
+      count_family(family);
       if (fused) *fused = fuse;
     }
   } else if (axis == 1) {
@@ -725,7 +712,9 @@ int launch_nt(const Conv1dArgs &base, int axis, const double *taps_host, int nta
     constexpr int kMinBlocks = NT <= 33 ? 4 : 2;
     a.strip = t.col_rot * NT + 1;   // strip + NT - 1 is a whole number of rotations
     dim3 grid((a.rc + kThreads - 1) / kThreads, (a.height + a.strip - 1) / a.strip);
+    if (grid.y > 65535) return MB200_EUNSUPPORTED;
     conv_col_kernel<NT, MODE, kThreads, kMinBlocks><<<grid, kThreads, 0, stream>>>(a, taps);
+    count_family(kConvGeneric);
   } else {
     constexpr int kMinBlocks = NT <= 33 ? 4 : 2;
     // strip + NT - 1 is a whole number of rotations and the strip is at least ~64 outputs
@@ -735,10 +724,12 @@ int launch_nt(const Conv1dArgs &base, int axis, const double *taps_host, int nta
     a.pitch = a.seg_w | 1;
     const int rows_per_cta = 4 * (32 / a.channels);
     const size_t smem = static_cast<size_t>(rows_per_cta) * a.pitch * a.channels * sizeof(float);
+    dim3 grid((a.width + a.strip - 1) / a.strip, (a.height + rows_per_cta - 1) / rows_per_cta);
+    if (smem > 200 * 1024 || grid.y > 65535) return MB200_EUNSUPPORTED;
     if (smem > 48 * 1024)            // per device attribute: set on every launch that needs it (a few microseconds)
       cudaFuncSetAttribute(conv_row_kernel<NT, MODE, kMinBlocks>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-    dim3 grid((a.width + a.strip - 1) / a.strip, (a.height + rows_per_cta - 1) / rows_per_cta);
     conv_row_kernel<NT, MODE, kMinBlocks><<<grid, 128, smem, stream>>>(a, taps);
+    count_family(kConvGeneric);
   }
   count_launch();
   const cudaError_t e = cudaGetLastError();

@@ -353,38 +353,33 @@ __global__ void __launch_bounds__(128, MINB) conv_mma_kernel(const MmaArgs a, co
   output(prev, epi_prev, prev_valid);
 }
 
-struct MmaTuning {
-  int enable, strip, minb, l2pf;
-  MmaTuning() {
-    auto get = [](const char *name, int fallback) {
-      const char *v = getenv(name);
-      return (v && *v) ? atoi(v) : fallback;
-    };
-    enable = get("MB200_MMA", -1);      // -1: automatic (float in / float out passes), 0: never, 1: whenever possible
-    strip = get("MB200_MMA_STRIP", 512);
-    minb = get("MB200_MMA_MINB", 4);
-    l2pf = get("MB200_MMA_L2PF", -1);    // -1: windows of <= 9 taps (measured: 9 taps 1.05 -> 0.98 ms, 25 taps 1.37 -> 1.40 ms)
+struct MmaSwitch {
+  std::atomic<int> enable;
+  MmaSwitch() {
+    const char *v = getenv("MB200_MMA");
+    enable = (v && *v) ? atoi(v) : -1;      // -1: automatic (float in / float out passes), 0: never, 1: whenever possible
   }
 };
-MmaTuning &mma_tuning() {
-  static MmaTuning t;
+MmaSwitch &mma_switch() {
+  static MmaSwitch t;
   return t;
 }
 std::atomic<unsigned long long> g_mma_launches{0};
 
 template <int NKS, int AXIS, int IO, int EPI>
-int launch_one(const MmaArgs &a, const MmaTaps<NKS> &taps, cudaStream_t stream) {
+int launch_one(const MmaArgs &a, const MmaTaps<NKS> &taps, int minb, cudaStream_t stream) {
   constexpr int NB = (4 * NKS - 8) / 8 + 2, RR = 8 * NB;
   constexpr int kWarpDoubles = AXIS == 1 ? RR * 36 : 16 * (2 * RR + 8);
   constexpr size_t smem = 4 * kWarpDoubles * sizeof(double);
   dim3 grid;
   if (AXIS == 1) grid = dim3((a.width + 31) / 32, (a.height + a.strip - 1) / a.strip);
   else grid = dim3((a.width + a.strip - 1) / a.strip, (a.height + 31) / 32);
+  if (grid.y > 65535) return MB200_EUNSUPPORTED;
   auto go = [&](auto kernel) {
     if (smem > 48 * 1024) cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
     kernel<<<grid, 128, smem, stream>>>(a, taps);
   };
-  if (mma_tuning().minb >= 4) go(conv_mma_kernel<NKS, AXIS, IO, EPI, 4>);
+  if (minb >= 4) go(conv_mma_kernel<NKS, AXIS, IO, EPI, 4>);
   else go(conv_mma_kernel<NKS, AXIS, IO, EPI, 3>);
   count_launch();
   g_mma_launches.fetch_add(1, std::memory_order_relaxed);
@@ -394,24 +389,24 @@ int launch_one(const MmaArgs &a, const MmaTaps<NKS> &taps, cudaStream_t stream) 
 }
 
 template <int NKS>
-int launch_nks(const MmaArgs &a, const double *taps_host, int axis, int io, bool epi, cudaStream_t stream) {
+int launch_nks(const MmaArgs &a, const double *taps_host, int axis, int io, bool epi, int minb, cudaStream_t stream) {
   MmaTaps<NKS> taps;
   for (int i = 0; i < 4 * NKS; ++i) taps.k[i] = i < a.ntaps ? taps_host[i] : 0.0;
   if (axis == 1) {
-    if (io == 1) return launch_one<NKS, 1, 1, 0>(a, taps, stream);
-    if (io == 2) return launch_one<NKS, 1, 2, 0>(a, taps, stream);
-    if (epi) return launch_one<NKS, 1, 0, 1>(a, taps, stream);
-    return launch_one<NKS, 1, 0, 0>(a, taps, stream);
+    if (io == 1) return launch_one<NKS, 1, 1, 0>(a, taps, minb, stream);
+    if (io == 2) return launch_one<NKS, 1, 2, 0>(a, taps, minb, stream);
+    if (epi) return launch_one<NKS, 1, 0, 1>(a, taps, minb, stream);
+    return launch_one<NKS, 1, 0, 0>(a, taps, minb, stream);
   }
-  if (io == 1) return launch_one<NKS, 0, 1, 0>(a, taps, stream);
-  if (io == 2) return launch_one<NKS, 0, 2, 0>(a, taps, stream);
-  return launch_one<NKS, 0, 0, 0>(a, taps, stream);
+  if (io == 1) return launch_one<NKS, 0, 1, 0>(a, taps, minb, stream);
+  if (io == 2) return launch_one<NKS, 0, 2, 0>(a, taps, minb, stream);
+  return launch_one<NKS, 0, 0, 0>(a, taps, minb, stream);
 }
 
 }  // namespace
 
-void set_conv_mma(int enable) { mma_tuning().enable = enable; }
-int conv_mma_enabled() { return mma_tuning().enable; }
+void set_conv_mma(int enable) { mma_switch().enable = enable; }
+int conv_mma_enabled() { return mma_switch().enable; }
 unsigned long long conv_mma_launches() { return g_mma_launches.load(std::memory_order_relaxed); }
 
 // RGBA, bias 0, 16-byte aligned images, <= 33 taps.  MB200_EUNSUPPORTED => the caller uses the DFMA kernels of conv1d.cu.
@@ -421,7 +416,7 @@ int launch_conv_mma(const void *src, void *dst, size_t width, size_t height, int
   // Default (-1): every float-in / float-out pass of <= 33 taps: one DMMA carries 256 FMAs where the DFMA kernels are
   // bound by issue slots next to the FP64 pipe (the two paths have not been timed against each other on the H100).  The rank-1 passes with a double intermediate (io 1 / 2) keep the DFMA
   // kernels.
-  const int mode = mma_tuning().enable;
+  const int mode = mma_switch().enable;
   if (mode == 0 || (mode < 0 && io != 0)) return MB200_EUNSUPPORTED;
   if (ntaps < 1 || ntaps > 33 || width * 32 > 0x7fffffffull || height > 0x3fffffffull) return MB200_EUNSUPPORTED;
   if (((reinterpret_cast<uintptr_t>(src) | reinterpret_cast<uintptr_t>(dst)) & 15) != 0) return MB200_EUNSUPPORTED;
@@ -430,16 +425,18 @@ int launch_conv_mma(const void *src, void *dst, size_t width, size_t height, int
   a.width = static_cast<int>(width); a.height = static_cast<int>(height);
   a.off = origin_offset;
   a.ntaps = ntaps;
-  a.strip = (mma_tuning().strip + 7) & ~7;
-  a.l2pf = mma_tuning().l2pf < 0 ? (ntaps <= 9 ? 1 : 0) : mma_tuning().l2pf;
+  const TuningKnobs knobs = tuning_knobs();
+  a.strip = (knobs.mma_strip + 7) & ~7;
+  // -1: windows of <= 9 taps (measured: 9 taps 1.05 -> 0.98 ms, 25 taps 1.37 -> 1.40 ms)
+  a.l2pf = knobs.mma_l2pf < 0 ? (ntaps <= 9 ? 1 : 0) : knobs.mma_l2pf;
   const bool epi = axis == 1 && io == 0 && epilogue && epilogue->source && (reinterpret_cast<uintptr_t>(epilogue->source) & 15) == 0;
   if (epi) { a.aux = epilogue->source; a.gain = epilogue->gain; a.qthreshold = epilogue->quantum_threshold; }
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   int rc;
-  if (ntaps <= 9) rc = launch_nks<4>(a, taps, axis, io, epi, s);
-  else if (ntaps <= 17) rc = launch_nks<6>(a, taps, axis, io, epi, s);
-  else if (ntaps <= 25) rc = launch_nks<8>(a, taps, axis, io, epi, s);
-  else rc = launch_nks<10>(a, taps, axis, io, epi, s);
+  if (ntaps <= 9) rc = launch_nks<4>(a, taps, axis, io, epi, knobs.mma_minb, s);
+  else if (ntaps <= 17) rc = launch_nks<6>(a, taps, axis, io, epi, knobs.mma_minb, s);
+  else if (ntaps <= 25) rc = launch_nks<8>(a, taps, axis, io, epi, knobs.mma_minb, s);
+  else rc = launch_nks<10>(a, taps, axis, io, epi, knobs.mma_minb, s);
   if (rc == MB200_OK && epilogue_fused) *epilogue_fused = epi;
   return rc;
 }

@@ -15,6 +15,29 @@ int fail(int code, const char *fmt, ...);       // records thread-local message,
 int cuda_fail(int cuda_error, const char *what); // wraps a cudaError_t
 void count_launch(unsigned n = 1);
 
+// ---- developer tuning knobs (runtime.cu, DESIGN §10) -------------------------
+// Initialised from MB200_<NAME> (an invalid value falls back to the default), settable with mb200_set_option("<name>").
+// Launchers take a snapshot per launch.
+struct TuningKnobs {
+  int mma_strip, mma_minb, mma_l2pf;                                  // conv_mma.cu
+  int pair, pair_async, pair_async_col, col_rot, row_pair_rot, row_rot;   // conv1d.cu
+  int resize_tma, resize_chunk, resize_slots, resize_strip;           // resize_stream.cu
+};
+TuningKnobs tuning_knobs();
+// MB200_OK; MB200_EINVAL for a value outside the knob's range; MB200_EUNSUPPORTED for a name that is not a knob
+int set_tuning_knob(const char *name, int value);
+bool get_tuning_knob(const char *name, int *value);
+
+// ---- per-family launch counters (runtime.cu): bumped where a family's kernel is launched, never on a decline -------
+enum LaunchFamily {
+  kConvPair, kConvPairAsync, kConvGeneric,                             // conv1d.cu
+  kResizeVStream, kResizeHTma, kResizeHStream,                         // resize_stream.cu
+  kResizeRegular, kResizeGather,                                       // resize.cu
+  kLaunchFamilies
+};
+void count_family(LaunchFamily family);
+bool get_family_count(const char *name, int *value);       // "<family>_launches"
+
 // ---- per-device state (runtime.cu) -----------------------------------------
 struct DeviceState;
 int ensure_device();                     // lazily initialises the current device; 0 or error

@@ -394,6 +394,7 @@ int launch_resize_axis(const float *src, size_t width, size_t height, int channe
     }
     if (rc == MB200_OK) {
       count_launch();
+      count_family(kResizeRegular);
       const cudaError_t e = cudaGetLastError();
       if (e != cudaSuccess) return cuda_fail(e, "resize launch");
       return MB200_OK;
@@ -419,6 +420,7 @@ int launch_resize_axis(const float *src, size_t width, size_t height, int channe
     }
   }
   count_launch();
+  count_family(kResizeGather);
   const cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return cuda_fail(e, "resize launch");
   return MB200_OK;

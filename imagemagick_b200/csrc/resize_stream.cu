@@ -691,15 +691,8 @@ namespace {
 
 template <int S, int N>
 int launch_sn(StreamArgs a, int axis, cudaStream_t s) {
-  static int strip_env = -1, slots_env = -1, chunk_env = 0;
-  if (strip_env < 0) {
-    const char *g = std::getenv("MB200_RESIZE_CHUNK");
-    chunk_env = g ? std::atoi(g) : 16;      // 16384^2 -> 8192^2: 2.02 ms with 128-byte chunks, 1.83 ms with 256-byte chunks
-    const char *e = std::getenv("MB200_RESIZE_STRIP");
-    strip_env = e ? std::atoi(e) : 0;
-    const char *f = std::getenv("MB200_RESIZE_SLOTS");
-    slots_env = f ? std::atoi(f) : 0;
-  }
+  // MB200_RESIZE_CHUNK: 16384^2 -> 8192^2: 2.02 ms with 128-byte chunks, 1.83 ms with 256-byte chunks (the default)
+  const TuningKnobs knobs = tuning_knobs();
   const int lanes_blocks = axis == 1 ? (a.width + 127) / 128 : (a.height + 127) / 128;
   int total = 0;
   for (int k = 0; k < a.nseg; ++k) total += a.seg_n[k];
@@ -708,7 +701,7 @@ int launch_sn(StreamArgs a, int axis, cudaStream_t s) {
   const int want = (8 * sm_count() * 3 + lanes_blocks - 1) / lanes_blocks;
   int strip = (total + want - 1) / want;
   if (strip < 24) strip = 24;
-  if (strip_env > 0) strip = strip_env;
+  if (knobs.resize_strip > 0) strip = knobs.resize_strip;
   a.strip = strip;
   int nstrips = 0;
   for (int k = 0; k < a.nseg; ++k) {
@@ -719,12 +712,14 @@ int launch_sn(StreamArgs a, int axis, cudaStream_t s) {
   nstrips += a.nborder;
   if (nstrips <= 0 || nstrips > 65535 || lanes_blocks > 65535) return MB200_EUNSUPPORTED;
   // default: the TMA-staged ring (110 instead of 168 registers, no bank-conflicted ring writes).  0 = the cp.async ring.
-  static const int tma_env = [] { const char *t = std::getenv("MB200_RESIZE_TMA"); return t ? std::atoi(t) : 1; }();
+  const int tma = knobs.resize_tma, chunk = knobs.resize_chunk, slots = knobs.resize_slots;
+  LaunchFamily family = kResizeHStream;
   CUtensorMap tmap;
-  if (axis == 0 && tma_env != 0 && (reinterpret_cast<uintptr_t>(a.src) & 15) == 0 &&
+  if (axis == 0 && tma != 0 && (reinterpret_cast<uintptr_t>(a.src) & 15) == 0 &&
       make_row_tensor_map(a.src, a.width, a.height, &tmap)) {
-    // TMA-staged ring: 3 slots x 8 KB per warp, 2 CTAs / SM (tma_env == 2: 2 slots, 3 CTAs / SM)
-    if (tma_env == 2) {
+    // TMA-staged ring: 3 slots x 8 KB per warp, 2 CTAs / SM (tma == 2: 2 slots, 3 CTAs / SM)
+    family = kResizeHTma;
+    if (tma == 2) {
       constexpr int smem = 4 * 2 * 8192 + 1024;
       cudaFuncSetAttribute(resize_h_tma_kernel<S, N, 2, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
       resize_h_tma_kernel<S, N, 2, 3><<<dim3(nstrips, lanes_blocks), 128, smem, s>>>(a, tmap);
@@ -734,16 +729,17 @@ int launch_sn(StreamArgs a, int axis, cudaStream_t s) {
       resize_h_tma_kernel<S, N, 3, 2><<<dim3(nstrips, lanes_blocks), 128, smem, s>>>(a, tmap);
     }
   } else if (axis == 1) {
+    family = kResizeVStream;
     resize_v_stream_kernel<S, N><<<dim3(lanes_blocks, nstrips), 128, 0, s>>>(a);
-  } else if (chunk_env == 16 && slots_env == 2) {  // experiment: 256-byte chunks, 2-slot rings, 3 CTAs / SM
+  } else if (chunk == 16 && slots == 2) {  // experiment: 256-byte chunks, 2-slot rings, 3 CTAs / SM
     constexpr int smem = 4 * 2 * HRing<16>::kSlotBytes;
     cudaFuncSetAttribute(resize_h_stream_kernel<S, N, 2, 3, 16>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     resize_h_stream_kernel<S, N, 2, 3, 16><<<dim3(nstrips, lanes_blocks), 128, smem, s>>>(a);
-  } else if (chunk_env == 16) {                    // 256-byte chunks, 3-slot rings, 2 CTAs / SM
+  } else if (chunk == 16) {                    // 256-byte chunks, 3-slot rings, 2 CTAs / SM
     constexpr int smem = 4 * 3 * HRing<16>::kSlotBytes;
     cudaFuncSetAttribute(resize_h_stream_kernel<S, N, 3, 2, 16>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);   // per device; cheap
     resize_h_stream_kernel<S, N, 3, 2, 16><<<dim3(nstrips, lanes_blocks), 128, smem, s>>>(a);
-  } else if (slots_env == 3) {                     // 4 CTAs / SM, 3-slot rings (221 KB of shared memory per SM)
+  } else if (slots == 3) {                     // 4 CTAs / SM, 3-slot rings (221 KB of shared memory per SM)
     constexpr int smem = 4 * 3 * HRing<8>::kSlotBytes;
     cudaFuncSetAttribute(resize_h_stream_kernel<S, N, 3, 4, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     resize_h_stream_kernel<S, N, 3, 4, 8><<<dim3(nstrips, lanes_blocks), 128, smem, s>>>(a);
@@ -752,6 +748,7 @@ int launch_sn(StreamArgs a, int axis, cudaStream_t s) {
     cudaFuncSetAttribute(resize_h_stream_kernel<S, N, 4, 3, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     resize_h_stream_kernel<S, N, 4, 3, 8><<<dim3(nstrips, lanes_blocks), 128, smem, s>>>(a);
   }
+  count_family(family);
   return MB200_OK;
 }
 

@@ -9,8 +9,12 @@
 #include <cuda_runtime.h>
 
 #include <atomic>
+#include <cctype>
+#include <climits>
 #include <cstdarg>
 #include <cstdio>
+#include <cstdlib>
+#include <cstring>
 #include <mutex>
 
 namespace mb200 {
@@ -51,6 +55,101 @@ int cuda_fail(int e, const char *what) {
 }
 
 void count_launch(unsigned n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
+
+namespace {
+// One row per knob: the option name (the environment variable is MB200_ + its upper-case form), the default and the
+// accepted values.  The upper bounds keep the strip arithmetic of the launchers inside int.
+constexpr int kKnobMax = 1 << 20;
+struct KnobSpec {
+  const char *name;
+  int TuningKnobs::*field;
+  int fallback;
+  bool (*valid)(int);
+};
+const KnobSpec kKnobs[] = {
+    {"mma_strip", &TuningKnobs::mma_strip, 512, [](int v) { return v >= 8 && v <= kKnobMax; }},   // rounded up to 8
+    {"mma_minb", &TuningKnobs::mma_minb, 4, [](int v) { return v == 3 || v == 4; }},
+    {"mma_l2pf", &TuningKnobs::mma_l2pf, -1, [](int v) { return v >= -1 && v <= 1; }},    // -1: windows of <= 9 taps
+    {"pair", &TuningKnobs::pair, 1, [](int v) { return v == 0 || v == 1; }},
+    {"pair_async", &TuningKnobs::pair_async, 1, [](int v) { return v == 0 || v == 1; }},
+    {"pair_async_col", &TuningKnobs::pair_async_col, -1, [](int v) { return v >= -1 && v <= 1; }},   // -1: < 33 taps
+    {"col_rot", &TuningKnobs::col_rot, 16, [](int v) { return v >= 1 && v <= kKnobMax; }},
+    {"row_pair_rot", &TuningKnobs::row_pair_rot, 16, [](int v) { return v >= 1 && v <= kKnobMax; }},
+    {"row_rot", &TuningKnobs::row_rot, 0, [](int v) { return v >= 0 && v <= kKnobMax; }},      // 0: >= 64 outputs
+    {"resize_tma", &TuningKnobs::resize_tma, 1, [](int v) { return v >= 0 && v <= 2; }},
+    {"resize_chunk", &TuningKnobs::resize_chunk, 16, [](int v) { return v == 8 || v == 16; }},
+    {"resize_slots", &TuningKnobs::resize_slots, 0, [](int v) { return v == 0 || v == 2 || v == 3; }},
+    {"resize_strip", &TuningKnobs::resize_strip, 0, [](int v) { return v >= 0 && v <= kKnobMax; }},  // 0: automatic
+};
+constexpr size_t kNumKnobs = sizeof(kKnobs) / sizeof(kKnobs[0]);
+
+struct KnobStore {
+  std::atomic<int> value[kNumKnobs];
+  KnobStore() {
+    for (size_t i = 0; i < kNumKnobs; ++i) {
+      char env[64] = "MB200_";
+      for (size_t j = 0; kKnobs[i].name[j] && j + 7 < sizeof(env); ++j)
+        env[6 + j] = static_cast<char>(std::toupper(static_cast<unsigned char>(kKnobs[i].name[j])));
+      int v = kKnobs[i].fallback;
+      const char *s = std::getenv(env);
+      if (s && *s) {
+        char *end = nullptr;
+        const long parsed = std::strtol(s, &end, 10);
+        if (*end == '\0' && parsed >= INT_MIN && parsed <= INT_MAX && kKnobs[i].valid(static_cast<int>(parsed)))
+          v = static_cast<int>(parsed);
+      }
+      value[i].store(v, std::memory_order_relaxed);
+    }
+  }
+};
+KnobStore &knob_store() {
+  static KnobStore s;
+  return s;
+}
+int knob_index(const char *name) {
+  for (size_t i = 0; i < kNumKnobs; ++i)
+    if (std::strcmp(kKnobs[i].name, name) == 0) return static_cast<int>(i);
+  return -1;
+}
+
+const char *const kFamilyNames[kLaunchFamilies] = {
+    "conv_pair_launches", "conv_pair_async_launches", "conv_generic_launches", "resize_v_stream_launches",
+    "resize_h_tma_launches", "resize_h_stream_launches", "resize_regular_launches", "resize_gather_launches"};
+std::atomic<unsigned long long> g_family_launches[kLaunchFamilies];
+}  // namespace
+
+TuningKnobs tuning_knobs() {
+  TuningKnobs t;
+  KnobStore &s = knob_store();
+  for (size_t i = 0; i < kNumKnobs; ++i) t.*kKnobs[i].field = s.value[i].load(std::memory_order_relaxed);
+  return t;
+}
+
+int set_tuning_knob(const char *name, int value) {
+  const int i = knob_index(name);
+  if (i < 0) return MB200_EUNSUPPORTED;
+  if (!kKnobs[i].valid(value)) return MB200_EINVAL;
+  knob_store().value[i].store(value, std::memory_order_relaxed);
+  return MB200_OK;
+}
+
+bool get_tuning_knob(const char *name, int *value) {
+  const int i = knob_index(name);
+  if (i < 0) return false;
+  *value = knob_store().value[i].load(std::memory_order_relaxed);
+  return true;
+}
+
+void count_family(LaunchFamily family) { g_family_launches[family].fetch_add(1, std::memory_order_relaxed); }
+
+bool get_family_count(const char *name, int *value) {
+  for (int f = 0; f < kLaunchFamilies; ++f)
+    if (std::strcmp(kFamilyNames[f], name) == 0) {
+      *value = static_cast<int>(g_family_launches[f].load(std::memory_order_relaxed) & 0x7fffffff);
+      return true;
+    }
+  return false;
+}
 
 int ensure_device() {
   int dev = -1;

@@ -569,13 +569,17 @@ def test_resize_streaming_kernels(filt, ratio, kind, monkeypatch):
     want = np.empty((oh, ow, 4), np.float32)
     assert oracle().orc_resize(P(src), w, h, 4, P(want), ow, oh, filt) == 0
     d = _dev(src)
+    families = ("resize_v_stream_launches", "resize_h_tma_launches", "resize_h_stream_launches")
     n0 = im.launch_count()
+    c0 = [util.get_option(f) for f in families]
     got = _host(im.ResizeImage(d, ow, oh, filt))
     streamed = im.launch_count() - n0
+    v, tma, cp = (util.get_option(f) - c for f, c in zip(families, c0))
     assert max_ulp(got, want) <= 1, (filt, ratio, kind)
     util.set_option("no_resize_stream", 1)
     ref = _host(im.ResizeImage(d, ow, oh, filt))
     assert streamed == 2                          # one launch per axis (borders ride along as extra CTAs)
+    assert v == 1 and tma + cp == 1               # ... and both are the streaming kernels, not the gather fallback
     assert max_ulp(got, ref) <= 1
     # only one axis reduced: the other axis is a 1:1 pass through the gather kernel
     util.set_option("no_resize_stream", 0)

@@ -106,9 +106,16 @@ def test_config3_strips_cover_the_whole_axis(axis):
     h, w = shape[0], shape[1]
     want = np.empty((h // 2, w // 2, 4), np.float32)
     assert oracle().orc_resize(P(src), w, h, 4, P(want), w // 2, h // 2, 22) == 0
+    families = ("resize_v_stream_launches", "resize_h_tma_launches", "resize_h_stream_launches", "resize_regular_launches",
+                "resize_gather_launches")
     n0 = im.launch_count()
+    c0 = [util.get_option(f) for f in families]
     got = _host(im.ResizeImage(_dev(src), w // 2, h // 2, im.LanczosFilter))
-    assert im.launch_count() - n0 == 2               # the streaming kernels (borders ride along)
+    assert im.launch_count() - n0 == 2
+    # the long axis on the streaming kernels (borders ride along), the 64 -> 32 axis (too short for the run detection)
+    # on the gather kernel
+    v, tma, cp, regular, gather = (util.get_option(f) - c for f, c in zip(families, c0))
+    assert (v, tma + cp) == ((0, 1) if axis == 0 else (1, 0)) and regular == 0 and gather == 1
     d = util.ulp_distance(got, want)
     assert d.max() <= 1
     assert (d == 0).mean() > 0.9999

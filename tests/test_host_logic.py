@@ -346,3 +346,69 @@ def test_scale_contribution_lists_reproduce_the_oracle(sizes):
     want = np.empty((oh, ow, 3), np.float32)
     assert util.oracle().orc_scale(util.P(src), w, h, 3, util.P(want), ow, oh) == 0
     assert np.array_equal(got, want)
+
+
+# ---- developer tuning knobs (DESIGN §10): validated in one place for mb200_set_option and the environment --------------
+KNOB_RANGES = {
+    "mma_strip": ([8, 9, 64, 512, 1 << 20], [0, -8, 7, (1 << 20) + 1]),
+    "mma_minb": ([3, 4], [0, 2, 5]),
+    "mma_l2pf": ([-1, 0, 1], [-2, 2]),
+    "pair": ([0, 1], [-1, 2]),
+    "pair_async": ([0, 1], [-1, 2]),
+    "pair_async_col": ([-1, 0, 1], [-2, 2]),
+    "col_rot": ([1, 3, 16], [0, -1]),
+    "row_pair_rot": ([1, 3, 16], [0, -1]),
+    "row_rot": ([0, 1, 5], [-1]),
+    "resize_tma": ([0, 1, 2], [-1, 3]),
+    "resize_chunk": ([8, 16], [0, 4, 12, 32]),
+    "resize_slots": ([0, 2, 3], [1, 4, -1]),
+    "resize_strip": ([0, 7, 24], [-1]),
+}
+COUNTERS = ["conv_mma_launches", "conv_pair_launches", "conv_pair_async_launches", "conv_generic_launches",
+            "resize_v_stream_launches", "resize_h_tma_launches", "resize_h_stream_launches", "resize_regular_launches",
+            "resize_gather_launches"]
+
+
+@pytest.mark.parametrize("name", sorted(KNOB_RANGES))
+def test_tuning_knobs_accept_their_range_only(name):
+    lib = _lib.load()
+    good, bad = KNOB_RANGES[name]
+    before = util.get_option(name)
+    for v in good:
+        util.set_option(name, v)
+        assert util.get_option(name) == v
+    for v in bad:
+        assert lib.mb200_set_option(name.encode(), v) == _lib.EINVAL, (name, v)
+        assert name in lib.mb200_last_error().decode()
+        assert util.get_option(name) == good[-1]          # a rejected value leaves the knob alone
+    util.set_option(name, before)
+
+
+def test_launch_counters_are_readable_and_not_settable():
+    lib = _lib.load()
+    for name in COUNTERS:
+        assert util.get_option(name) >= 0
+        assert lib.mb200_set_option(name.encode(), 0) == _lib.EINVAL
+    v = C.c_int()
+    assert lib.mb200_get_option(b"no_such_option", C.byref(v)) == _lib.EINVAL
+
+
+def test_invalid_environment_values_fall_back_to_the_defaults():
+    """MB200_MMA_STRIP=0 used to divide by zero in the launch grid and MB200_COL_ROT=0 to make one-row strips; an invalid
+    value is now ignored.  Run in a fresh process: the environment is read once."""
+    import os
+    import subprocess
+    import sys
+    env = dict(os.environ, MB200_MMA_STRIP="0", MB200_COL_ROT="0", MB200_ROW_PAIR_ROT="-3", MB200_MMA_MINB="7",
+               MB200_RESIZE_CHUNK="12", MB200_RESIZE_SLOTS="1", MB200_RESIZE_TMA="x", MB200_ROW_ROT="5",
+               MB200_RESIZE_STRIP="24", MB200_PAIR_ASYNC_COL="0")
+    code = ("import ctypes as C\nfrom imagemagick_b200 import _lib\nv = C.c_int()\n"
+            "for n in %r:\n    assert _lib.load().mb200_get_option(n.encode(), C.byref(v)) == 0\n"
+            "    print(n, v.value)\n" % [
+                "mma_strip", "col_rot", "row_pair_rot", "mma_minb", "resize_chunk", "resize_slots", "resize_tma",
+                "row_rot", "resize_strip", "pair_async_col"])
+    p = subprocess.run([sys.executable, "-c", code], env=env, cwd=str(ROOT), capture_output=True, text=True, timeout=120)
+    assert p.returncode == 0, p.stderr
+    got = dict(line.split() for line in p.stdout.split("\n") if line)
+    assert got == {"mma_strip": "512", "col_rot": "16", "row_pair_rot": "16", "mma_minb": "4", "resize_chunk": "16",
+                   "resize_slots": "0", "resize_tma": "1", "row_rot": "5", "resize_strip": "24", "pair_async_col": "0"}

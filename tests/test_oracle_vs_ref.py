@@ -477,3 +477,36 @@ def test_adaptive_blur_and_sharpen_bit_exact(ch, fn, args):
     a = np.empty_like(src)
     assert getattr(util.oracle(), "orc_" + fn)(util.P(src), util.P(a), 75, 52, ch, *args) == 0
     assert digest(a) == reference("", lambda: ref_out(fn, src, src.shape, args))
+
+
+def _taps_string(values):
+    return ",".join(repr(float(v)) for v in values)
+
+
+# 1-D kernels (rows Nx1, columns 1xN): asymmetric, off-centre, mixed-sign, zero-sum, NaN cells, even lengths, the
+# built-in one-sided comet, and windows on both sides of the 9 / 17 / 33 / 65 tap template boundaries of the GPU kernels
+ONE_D_KERNELS = ["5x1+0+0: 1,2,3,4,5", "1x5+0+4: 1,-2,3,-4,0.5", "4x1: 1,2,3,4", "1x4+0+2: 0.5,1,-1,2",
+                 "1x5: 1,nan,2,3,4", "5x1: 1,2,nan,3,4", "7x1+6+0: 1,-1,1,-1,1,-1,1", "3x1: -1,0,1", "1x3: -1,0,1",
+                 "1x1: 2", "comet:0x2", "comet:0x3+90", "comet:0x2;comet:0x2+90"]
+for _n in (9, 10, 17, 18, 33, 34, 65, 66):
+    _i = np.arange(_n)
+    _mixed = ((5 * _i) % 9 - 4) / 4.0
+    _mixed[0] = 1.25
+    _zero = ((7 * _i) % 11 - 5) / 4.0
+    _zero[-1] = -_zero[:-1].sum()
+    ONE_D_KERNELS += [f"{_n}x1+{_n - 1}+0: {_taps_string(_mixed)}", f"1x{_n}+0+{_n // 2}: {_taps_string(_zero)}"]
+
+
+@pytest.mark.parametrize("name", ONE_D_KERNELS)
+def test_one_d_kernels_convolve_correlate_bit_exact(name):
+    """Convolve reflects a 1-D kernel and its origin (morphology.c:2612-2626), Correlate rotates it first (:3779-3793);
+    a width-1 kernel with NaN cells takes the column path that scales gamma by height / count (:2654-2807).  Zero-sum
+    taps give PerceptibleReciprocal a weight sum near zero of either sign."""
+    kernels = kernel_list(name)
+    for ch in (1, 2, 3, 4):
+        for kind in ("noise", "alpha_blocks", "hdr"):
+            src = make_image(53, 37, ch, seed=31 + ch, kind=kind)
+            for method in (1, 2):
+                b = util.orc_morphology(src, method, 1, kernels)
+                assert digest(b) == reference(f"{ch},{kind},{method}", lambda: ref_morphology(src, method, 1, name)), \
+                    (name, ch, kind, method)
