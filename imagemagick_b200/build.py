@@ -25,8 +25,8 @@ ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC,-fvisibility=hidden,-ffp-contract=off",
               "-Xptxas", "-v"]
 
-SOURCES = ["runtime.cu", "kernel_info.cpp", "resize_filter.cpp", "conv1d.cu", "conv_mma.cu", "morph2d.cu", "morph_stream.cu", "cache.cu",
-           "resize.cu", "resize_stream.cu", "colorspace.cu", "hexcone.cu", "pointwise.cu", "equalize.cu", "stencils.cu", "api.cu"]
+SOURCES = ["runtime.cu", "kernel_info.cpp", "resize_filter.cpp", "resize_tables.cpp", "conv1d.cu", "conv_mma.cu",
+           "morph2d.cu", "morph_stream.cu", "cache.cu", "resize.cu", "resize_stream.cu", "colorspace.cu", "hexcone.cu", "pointwise.cu", "equalize.cu", "stencils.cu", "api.cu"]
 
 
 def _nvcc() -> str:

@@ -33,9 +33,7 @@
 
 #include <cuda_runtime.h>
 
-#include <atomic>
 #include <cstdint>
-#include <cstdlib>
 
 namespace mb200 {
 namespace {
@@ -353,19 +351,6 @@ __global__ void __launch_bounds__(128, MINB) conv_mma_kernel(const MmaArgs a, co
   output(prev, epi_prev, prev_valid);
 }
 
-struct MmaSwitch {
-  std::atomic<int> enable;
-  MmaSwitch() {
-    const char *v = getenv("MB200_MMA");
-    enable = (v && *v) ? atoi(v) : -1;      // -1: automatic (float in / float out passes), 0: never, 1: whenever possible
-  }
-};
-MmaSwitch &mma_switch() {
-  static MmaSwitch t;
-  return t;
-}
-std::atomic<unsigned long long> g_mma_launches{0};
-
 template <int NKS, int AXIS, int IO, int EPI>
 int launch_one(const MmaArgs &a, const MmaTaps<NKS> &taps, int minb, cudaStream_t stream) {
   constexpr int NB = (4 * NKS - 8) / 8 + 2, RR = 8 * NB;
@@ -382,7 +367,7 @@ int launch_one(const MmaArgs &a, const MmaTaps<NKS> &taps, int minb, cudaStream_
   if (minb >= 4) go(conv_mma_kernel<NKS, AXIS, IO, EPI, 4>);
   else go(conv_mma_kernel<NKS, AXIS, IO, EPI, 3>);
   count_launch();
-  g_mma_launches.fetch_add(1, std::memory_order_relaxed);
+  count_family(kConvMma);
   const cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return cuda_fail(e, "conv_mma launch");
   return MB200_OK;
@@ -405,10 +390,6 @@ int launch_nks(const MmaArgs &a, const double *taps_host, int axis, int io, bool
 
 }  // namespace
 
-void set_conv_mma(int enable) { mma_switch().enable = enable; }
-int conv_mma_enabled() { return mma_switch().enable; }
-unsigned long long conv_mma_launches() { return g_mma_launches.load(std::memory_order_relaxed); }
-
 // RGBA, bias 0, 16-byte aligned images, <= 33 taps.  MB200_EUNSUPPORTED => the caller uses the DFMA kernels of conv1d.cu.
 int launch_conv_mma(const void *src, void *dst, size_t width, size_t height, int axis, const double *taps, int ntaps,
                     int origin_offset, void *stream, int io, const UnsharpEpilogue *epilogue, bool *epilogue_fused) {
@@ -416,7 +397,8 @@ int launch_conv_mma(const void *src, void *dst, size_t width, size_t height, int
   // Default (-1): every float-in / float-out pass of <= 33 taps: one DMMA carries 256 FMAs where the DFMA kernels are
   // bound by issue slots next to the FP64 pipe (the two paths have not been timed against each other on the H100).  The rank-1 passes with a double intermediate (io 1 / 2) keep the DFMA
   // kernels.
-  const int mode = mma_switch().enable;
+  const TuningKnobs knobs = tuning_knobs();
+  const int mode = knobs.conv_mma;
   if (mode == 0 || (mode < 0 && io != 0)) return MB200_EUNSUPPORTED;
   if (ntaps < 1 || ntaps > 33 || width * 32 > 0x7fffffffull || height > 0x3fffffffull) return MB200_EUNSUPPORTED;
   if (((reinterpret_cast<uintptr_t>(src) | reinterpret_cast<uintptr_t>(dst)) & 15) != 0) return MB200_EUNSUPPORTED;
@@ -425,7 +407,6 @@ int launch_conv_mma(const void *src, void *dst, size_t width, size_t height, int
   a.width = static_cast<int>(width); a.height = static_cast<int>(height);
   a.off = origin_offset;
   a.ntaps = ntaps;
-  const TuningKnobs knobs = tuning_knobs();
   a.strip = (knobs.mma_strip + 7) & ~7;
   // -1: windows of <= 9 taps (measured: 9 taps 1.05 -> 0.98 ms, 25 taps 1.37 -> 1.40 ms)
   a.l2pf = knobs.mma_l2pf < 0 ? (ntaps <= 9 ? 1 : 0) : knobs.mma_l2pf;

@@ -505,6 +505,13 @@ namespace mb200 {
 void rotate_kernel_info(mb200_kernel_info *k, double angle) {
   for (; k; k = k->next) rotate_kernel(k, angle);
 }
+
+KernelList blur_kernel_pair(double radius, double sigma) {
+  KernelList k(mb200_acquire_kernel_builtin(MB200_BlurKernel, radius, sigma, 0.0, 0.0));
+  if (k) k->next = mb200_acquire_kernel_builtin(MB200_BlurKernel, radius, sigma, 90.0, 0.0);
+  if (k && !k->next) k.reset();
+  return k;
+}
 }  // namespace mb200
 
 extern "C" {

@@ -5,8 +5,12 @@
 
 #include <cstddef>
 #include <cstdint>
+#include <memory>
 
 struct CUmemPoolHandle_st;      // cudaMemPool_t == CUmemPoolHandle_st * (driver_types.h)
+
+// resize_filter.cpp: the source sample a Copy-trait channel takes for every output of one axis (resize.c:3697-3707)
+extern "C" int mb200_resize_nearest(int filter, size_t in_n, size_t out_n, double factor, long *nearest);
 
 namespace mb200 {
 
@@ -15,28 +19,27 @@ int fail(int code, const char *fmt, ...);       // records thread-local message,
 int cuda_fail(int cuda_error, const char *what); // wraps a cudaError_t
 void count_launch(unsigned n = 1);
 
-// ---- developer tuning knobs (runtime.cu, DESIGN §10) -------------------------
-// Initialised from MB200_<NAME> (an invalid value falls back to the default), settable with mb200_set_option("<name>").
-// Launchers take a snapshot per launch.
+// ---- run-time options (runtime.cu, DESIGN §10) ---------------------------------
+// Initialised from the environment (an invalid value falls back to the default), settable with
+// mb200_set_option("<name>").  Callers take a snapshot per call.
 struct TuningKnobs {
-  int mma_strip, mma_minb, mma_l2pf;                                  // conv_mma.cu
+  int mma_strip, mma_minb, mma_l2pf, conv_mma;                        // conv_mma.cu
   int pair, pair_async, pair_async_col, col_rot, row_pair_rot, row_rot;   // conv1d.cu
   int resize_tma, resize_chunk, resize_slots, resize_strip;           // resize_stream.cu
+  // switches (0 / 1) that force the generic paths, or opt in to a slower one, in api.cu
+  int no_rank1, no_morph_stream, no_resize_stream, resize_regular_h, no_fused_unsharp, resize_fused;
 };
 TuningKnobs tuning_knobs();
-// MB200_OK; MB200_EINVAL for a value outside the knob's range; MB200_EUNSUPPORTED for a name that is not a knob
-int set_tuning_knob(const char *name, int value);
-bool get_tuning_knob(const char *name, int *value);
 
 // ---- per-family launch counters (runtime.cu): bumped where a family's kernel is launched, never on a decline -------
 enum LaunchFamily {
+  kConvMma,                                                            // conv_mma.cu
   kConvPair, kConvPairAsync, kConvGeneric,                             // conv1d.cu
   kResizeVStream, kResizeHTma, kResizeHStream,                         // resize_stream.cu
   kResizeRegular, kResizeGather,                                       // resize.cu
   kLaunchFamilies
 };
 void count_family(LaunchFamily family);
-bool get_family_count(const char *name, int *value);       // "<family>_launches"
 
 // ---- per-device state (runtime.cu) -----------------------------------------
 struct DeviceState;
@@ -68,6 +71,12 @@ void release_stage(StageRef *ref, void *stream);
 
 // ---- kernel helpers (kernel_info.cpp) --------------------------------------
 void rotate_kernel_info(mb200_kernel_info *k, double angle);
+struct KernelInfoFree {
+  void operator()(mb200_kernel_info *k) const { mb200_destroy_kernel_info(k); }
+};
+using KernelList = std::unique_ptr<mb200_kernel_info, KernelInfoFree>;     // owns a whole kernel list
+// BlurImage's kernel list "blur:RxS;blur:RxS+90" (effect.c:788); null when out of memory
+KernelList blur_kernel_pair(double radius, double sigma);
 
 // ---- channel traits (pixel.c:6356-6381) ------------------------------------
 inline bool has_alpha(int channels) { return channels == 2 || channels == 4; }
@@ -94,9 +103,6 @@ int launch_conv1d(const float *src, float *dst, size_t width, size_t height, int
 int launch_conv_mma(const void *src, void *dst, size_t width, size_t height, int axis, const double *taps_window_order,
                     int ntaps, int origin_offset, void *stream, int io, const UnsharpEpilogue *epilogue,
                     bool *epilogue_fused);
-void set_conv_mma(int enable);
-int conv_mma_enabled();
-unsigned long long conv_mma_launches();
 
 // conv2d.cu: general 2-D convolution / erode / dilate (MorphologyPrimitive row path)
 int launch_morph2d(const float *src, float *dst, size_t width, size_t height, int channels,
@@ -108,29 +114,55 @@ int launch_morph2d(const float *src, float *dst, size_t width, size_t height, in
 int launch_morph_stream(const float *src, float *dst, size_t width, size_t height, int channels, int method,
                         const double *kernel_window_order, int kw, int kh, int ox, int oy, void *stream);
 
-// resize.cu: one axis of ResizeImage.  Contribution table lives in device memory.
-int launch_resize_axis(const float *src, size_t width, size_t height, int channels, float *dst,
-                       size_t out_n, int axis, const int *d_start, const int *d_count,
-                       const double *d_weights, int max_taps, int max_span, int reg_stride, int reg_taps,
-                       const double *d_wreg, void *stream, long o_begin = -1, long o_end = -1);
-
-// resize_stream.cu: streaming kernels for runs of outputs with bit-identical weights (integer-ratio
-// reductions, RGBA).  seg_*: first output / number of outputs / start[] of each run; d_wsets[nseg][taps];
-// d_border: the outputs outside the runs (gathered by extra CTAs of the same launch).
+// ---- resize axis tables (resize_tables.cpp) ---------------------------------
+// One axis of ResizeImage, planned on the host and resident on one device: the reference's contribution lists
+// (tap-major), and what the specialised kernels need on top of them.
 #define MB200_RESIZE_MAX_SEGMENTS 8
-int launch_resize_stream(const float *src, size_t width, size_t height, float *dst, size_t out_n, int axis,
-                         int stride, int taps, int nseg, const int *seg_o, const int *seg_n, const int *seg_src,
-                         const double *d_wsets, int nborder, const int *d_border, const int *d_start,
-                         const int *d_count, const double *d_weights, void *stream);
+struct ResizeAxis {
+  int device = -1, filter = 0;
+  mb200_filter_options options{};     // expert settings the table was built with (all zero: none)
+  size_t in_n = 0, out_n = 0;
+  long taps = 0;
+  // max_span: widest source span of any aligned block of 32 outputs (tile width of the tiled horizontal kernel)
+  int max_span = 0, reg_stride = 0, reg_taps = 0;
+  int *d_start = nullptr, *d_count = nullptr;
+  double *d_weights = nullptr;
+  double *d_wreg = nullptr;           // [out_n][reg_taps] when the interior is regular (integer-ratio reduction)
+  // streaming kernels (resize_stream.cu): runs of outputs with bit-identical weights, and the
+  // complement (borders, short runs) that stays with the gather kernels
+  int nseg = 0, seg_o[MB200_RESIZE_MAX_SEGMENTS], seg_n[MB200_RESIZE_MAX_SEGMENTS], seg_src[MB200_RESIZE_MAX_SEGMENTS];
+  double *d_wsets = nullptr;
+  int nborder = 0;
+  int *d_border = nullptr;
+  // fused V+H kernel (resize_stream.cu): the runs cut into tiles of tile_w (this axis used as x) / tile_h (as y) outputs
+  int *d_tiles_x = nullptr, *d_tiles_y = nullptr;
+  int ntiles_x = 0, ntiles_y = 0;
+  unsigned char *d_is_border = nullptr;       // [out_n]: output lies outside the runs
+  ResizeAxis() = default;
+  ResizeAxis(const ResizeAxis &) = delete;
+  ResizeAxis &operator=(const ResizeAxis &) = delete;
+  ~ResizeAxis();              // frees on the owning device; cudaFree waits for launches that still read the buffers
+};
+// The tables of (current device, filter, options, in_n, out_n), from a bounded cache shared by all threads.  The
+// returned reference keeps the tables alive while the caller's launches are queued, even if they are evicted meanwhile.
+int resize_axis_tables(int filter, const mb200_filter_options *options, size_t in_n, size_t out_n, double factor,
+                       std::shared_ptr<const ResizeAxis> *out);
+
+// resize.cu: one axis of ResizeImage on the gather kernels; `regular` allows the regular-stride kernels (when the
+// axis has them).
+int launch_resize_axis(const float *src, size_t width, size_t height, int channels, float *dst, int axis,
+                       const ResizeAxis &t, bool regular, void *stream);
+
+// resize_stream.cu: streaming kernels for the runs of outputs with bit-identical weights (integer-ratio
+// reductions, RGBA); extra CTAs of the same launch gather the outputs outside the runs.
+int launch_resize_stream(const float *src, size_t width, size_t height, float *dst, int axis, const ResizeAxis &t,
+                         void *stream);
 
 // Fused vertical + horizontal pass for equal integer reductions on both axes (RGBA): tile lists of both axes' runs,
 // the two-pass path's contribution / border lists for the outputs outside the runs.
 void resize_fused_tile(int stride, int taps, int *tile_w, int *tile_h);
-int launch_resize_fused(const float *src, size_t width, size_t height, float *dst, size_t out_w, size_t out_h, int stride,
-                        int taps, const int *d_xtiles, int nxt, const int *d_ytiles, int nyt, const double *d_wx,
-                        const double *d_wy, const int *d_xstart, const int *d_xcount, const double *d_xweights,
-                        const int *d_ystart, const int *d_ycount, const double *d_yweights, const int *d_xborder, int nxborder,
-                        const int *d_yborder, int nyborder, const unsigned char *d_row_is_border, void *stream);
+int launch_resize_fused(const float *src, size_t width, size_t height, float *dst, const ResizeAxis &x,
+                        const ResizeAxis &y, void *stream);
 
 // colorspace.cu
 int launch_colorspace(float *buf, size_t npixels, int channels, int from, int to, const mb200_colorspace_options *options,

@@ -363,10 +363,9 @@ int launch_regular_ch(const ResizeArgs &a, int axis, int stride, int ntaps, cons
 
 }  // namespace
 
-int launch_resize_axis(const float *src, size_t width, size_t height, int channels, float *dst, size_t out_n,
-                       int axis, const int *d_start, const int *d_count, const double *d_weights,
-                       int /*max_taps*/, int max_span, int reg_stride, int reg_taps, const double *d_wreg,
-                       void *stream, long o_begin, long o_end) {
+int launch_resize_axis(const float *src, size_t width, size_t height, int channels, float *dst, int axis,
+                       const ResizeAxis &t, bool regular, void *stream) {
+  const size_t out_n = t.out_n;
   if (width == 0 || height == 0 || out_n == 0 || channels < 1 || channels > 4)
     return fail(MB200_EINVAL, "resize: bad geometry");
   if (width > 0x3fffffffull || height > 0x3fffffffull || out_n > 0x3fffffffull)
@@ -376,21 +375,19 @@ int launch_resize_axis(const float *src, size_t width, size_t height, int channe
   a.src = src; a.dst = dst;
   a.width = static_cast<int>(width); a.height = static_cast<int>(height);
   a.out_n = static_cast<int>(out_n);
-  a.start = d_start; a.count = d_count; a.weights = d_weights;
+  a.start = t.d_start; a.count = t.d_count; a.weights = t.d_weights;
   a.lines_per_thread = 8;
   if (axis == 1) { a.out_w = a.width; a.out_h = a.out_n; }
   else { a.out_w = a.out_n; a.out_h = a.height; }
-  const bool whole = o_begin < 0;
-  a.o_begin = whole ? 0 : static_cast<int>(o_begin);
-  a.o_end = whole ? a.out_n : static_cast<int>(o_end);
-  if (a.o_begin >= a.o_end) return MB200_OK;
-  if (whole && reg_stride > 0 && d_wreg != nullptr) {
+  a.o_begin = 0;
+  a.o_end = a.out_n;
+  if (regular && t.d_wreg != nullptr) {
     int rc = MB200_EUNSUPPORTED;
     switch (channels) {
-      case 1: rc = launch_regular_ch<1>(a, axis, reg_stride, reg_taps, d_wreg, max_span, s); break;
-      case 2: rc = launch_regular_ch<2>(a, axis, reg_stride, reg_taps, d_wreg, max_span, s); break;
-      case 3: rc = launch_regular_ch<3>(a, axis, reg_stride, reg_taps, d_wreg, max_span, s); break;
-      default: rc = launch_regular_ch<4>(a, axis, reg_stride, reg_taps, d_wreg, max_span, s); break;
+      case 1: rc = launch_regular_ch<1>(a, axis, t.reg_stride, t.reg_taps, t.d_wreg, t.max_span, s); break;
+      case 2: rc = launch_regular_ch<2>(a, axis, t.reg_stride, t.reg_taps, t.d_wreg, t.max_span, s); break;
+      case 3: rc = launch_regular_ch<3>(a, axis, t.reg_stride, t.reg_taps, t.d_wreg, t.max_span, s); break;
+      default: rc = launch_regular_ch<4>(a, axis, t.reg_stride, t.reg_taps, t.d_wreg, t.max_span, s); break;
     }
     if (rc == MB200_OK) {
       count_launch();
@@ -401,7 +398,7 @@ int launch_resize_axis(const float *src, size_t width, size_t height, int channe
     }
   }
   if (axis == 1) {
-    dim3 grid((a.width + 127) / 128, (a.o_end - a.o_begin + a.lines_per_thread - 1) / a.lines_per_thread);
+    dim3 grid((a.width + 127) / 128, (a.out_n + a.lines_per_thread - 1) / a.lines_per_thread);
     if (grid.y > 65535) return fail(MB200_EINVAL, "resize: too many rows");
     switch (channels) {
       case 1: resize_vertical_kernel<1><<<grid, 128, 0, s>>>(a); break;
@@ -410,7 +407,7 @@ int launch_resize_axis(const float *src, size_t width, size_t height, int channe
       default: resize_vertical_kernel<4><<<grid, 128, 0, s>>>(a); break;
     }
   } else {
-    dim3 grid((a.o_end - a.o_begin + 127) / 128, (a.height + a.lines_per_thread - 1) / a.lines_per_thread);
+    dim3 grid((a.out_n + 127) / 128, (a.height + a.lines_per_thread - 1) / a.lines_per_thread);
     if (grid.y > 65535) return fail(MB200_EINVAL, "resize: too many rows");
     switch (channels) {
       case 1: resize_horizontal_kernel<1><<<grid, 128, 0, s>>>(a); break;

@@ -652,34 +652,34 @@ void resize_fused_tile(int stride, int taps, int *tw, int *th) {
   else if (stride == 2 && taps == 8) { *tw = FusedGeom<2, 8>::TW; *th = FusedGeom<2, 8>::TH; }
 }
 
-// Fused vertical + horizontal pass.  d_xtiles / d_ytiles: {o0, nout, src0, set} of every tile (4 ints each); the
-// contribution lists and border lists are the ones of the two-pass path.  MB200_EUNSUPPORTED => use two passes.
-int launch_resize_fused(const float *src, size_t width, size_t height, float *dst, size_t out_w, size_t out_h, int stride,
-                        int taps, const int *d_xtiles, int nxt, const int *d_ytiles, int nyt, const double *d_wx,
-                        const double *d_wy, const int *d_xstart, const int *d_xcount, const double *d_xweights,
-                        const int *d_ystart, const int *d_ycount, const double *d_yweights, const int *d_xborder, int nxborder,
-                        const int *d_yborder, int nyborder, const unsigned char *d_row_is_border, void *stream) {
+// Fused vertical + horizontal pass: the tiles of both axes' runs, then the two-pass path's contribution and border lists
+// for the outputs outside the runs.  MB200_EUNSUPPORTED => use two passes.
+int launch_resize_fused(const float *src, size_t width, size_t height, float *dst, const ResizeAxis &x,
+                        const ResizeAxis &y, void *stream) {
+  const int stride = x.reg_stride, taps = x.reg_taps, nxt = x.ntiles_x, nyt = y.ntiles_y;
+  if (y.reg_stride != stride || y.reg_taps != taps) return MB200_EUNSUPPORTED;
   if (width > 0x3fffffffull || height > 0x3fffffffull || nxt <= 0 || nyt <= 0 || nyt > 65535) return MB200_EUNSUPPORTED;
+  const size_t out_w = x.out_n, out_h = y.out_n;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   FusedArgs a{};
   a.src = src; a.dst = dst;
   a.width = static_cast<int>(width); a.height = static_cast<int>(height);
   a.out_w = static_cast<int>(out_w); a.out_h = static_cast<int>(out_h);
-  a.xt = reinterpret_cast<const Tile *>(d_xtiles); a.yt = reinterpret_cast<const Tile *>(d_ytiles);
-  a.wx = d_wx; a.wy = d_wy;
+  a.xt = reinterpret_cast<const Tile *>(x.d_tiles_x); a.yt = reinterpret_cast<const Tile *>(y.d_tiles_y);
+  a.wx = x.d_wsets; a.wy = y.d_wsets;
   int rc = MB200_EUNSUPPORTED;
   if (stride == 2 && taps == 12) rc = launch_fused_sn<2, 12>(a, nxt, nyt, s);
   else if (stride == 2 && taps == 8) rc = launch_fused_sn<2, 8>(a, nxt, nyt, s);
   if (rc != MB200_OK) return rc;
   count_launch();
-  if (nxborder > 0 || nyborder > 0) {
+  if (x.nborder > 0 || y.nborder > 0) {
     Border2dArgs b{};
     b.src = src; b.dst = dst; b.width = a.width; b.height = a.height; b.out_w = a.out_w; b.out_h = a.out_h;
-    b.xstart = d_xstart; b.xcount = d_xcount; b.ystart = d_ystart; b.ycount = d_ycount;
-    b.xweights = d_xweights; b.yweights = d_yweights;
-    b.xborder = d_xborder; b.yborder = d_yborder; b.nxborder = nxborder; b.nyborder = nyborder;
-    const size_t work = std::max(static_cast<size_t>(nyborder) * out_w, static_cast<size_t>(nxborder) * out_h);
-    resize_border2d_kernel<<<dim3(static_cast<unsigned>((work + 127) / 128), 2), 128, 0, s>>>(b, d_row_is_border);
+    b.xstart = x.d_start; b.xcount = x.d_count; b.ystart = y.d_start; b.ycount = y.d_count;
+    b.xweights = x.d_weights; b.yweights = y.d_weights;
+    b.xborder = x.d_border; b.yborder = y.d_border; b.nxborder = x.nborder; b.nyborder = y.nborder;
+    const size_t work = std::max(static_cast<size_t>(y.nborder) * out_w, static_cast<size_t>(x.nborder) * out_h);
+    resize_border2d_kernel<<<dim3(static_cast<unsigned>((work + 127) / 128), 2), 128, 0, s>>>(b, y.d_is_border);
     count_launch();
   }
   const cudaError_t e = cudaGetLastError();
@@ -754,24 +754,24 @@ int launch_sn(StreamArgs a, int axis, cudaStream_t s) {
 
 }  // namespace
 
-// Streams the uniform runs of one axis (RGBA only) and gathers the `nborder` remaining outputs in the
-// same launch.  MB200_EUNSUPPORTED => the caller uses the kernels of resize.cu for the whole axis.
-int launch_resize_stream(const float *src, size_t width, size_t height, float *dst, size_t out_n, int axis,
-                         int stride, int taps, int nseg, const int *seg_o, const int *seg_n, const int *seg_src,
-                         const double *d_wsets, int nborder, const int *d_border, const int *d_start,
-                         const int *d_count, const double *d_weights, void *stream) {
-  if (d_wsets == nullptr || nseg <= 0 || nseg > kMaxSegments) return MB200_EUNSUPPORTED;
+// Streams the uniform runs of one axis (RGBA only) and gathers the remaining outputs in the same launch.
+// MB200_EUNSUPPORTED => the caller uses the kernels of resize.cu for the whole axis.
+int launch_resize_stream(const float *src, size_t width, size_t height, float *dst, int axis, const ResizeAxis &t,
+                         void *stream) {
+  const size_t out_n = t.out_n;
+  const int stride = t.reg_stride, taps = t.reg_taps;
+  if (t.d_wsets == nullptr || t.nseg <= 0 || t.nseg > kMaxSegments) return MB200_EUNSUPPORTED;
   if (width > 0x3fffffffull || height > 0x3fffffffull || out_n > 0x3fffffffull) return MB200_EUNSUPPORTED;
   StreamArgs a{};
   a.src = src; a.dst = dst;
   a.width = static_cast<int>(width); a.height = static_cast<int>(height);
   if (axis == 1) { a.out_w = a.width; a.out_h = static_cast<int>(out_n); a.in_n = a.height; }
   else { a.out_w = static_cast<int>(out_n); a.out_h = a.height; a.in_n = a.width; }
-  a.nseg = nseg;
-  for (int k = 0; k < nseg; ++k) { a.seg_o[k] = seg_o[k]; a.seg_n[k] = seg_n[k]; a.seg_src[k] = seg_src[k]; }
-  a.wsets = d_wsets;
-  a.nborder = nborder; a.border = d_border; a.out_n = static_cast<int>(out_n);
-  a.start = d_start; a.count = d_count; a.weights = d_weights;
+  a.nseg = t.nseg;
+  for (int k = 0; k < t.nseg; ++k) { a.seg_o[k] = t.seg_o[k]; a.seg_n[k] = t.seg_n[k]; a.seg_src[k] = t.seg_src[k]; }
+  a.wsets = t.d_wsets;
+  a.nborder = t.nborder; a.border = t.d_border; a.out_n = static_cast<int>(out_n);
+  a.start = t.d_start; a.count = t.d_count; a.weights = t.d_weights;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   int rc = MB200_EUNSUPPORTED;
   if (stride == 2 && taps == 12) rc = launch_sn<2, 12>(a, axis, s);        // 3-lobe filters, 2x

@@ -57,19 +57,29 @@ int cuda_fail(int e, const char *what) {
 void count_launch(unsigned n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
 
 namespace {
-// One row per knob: the option name (the environment variable is MB200_ + its upper-case form), the default and the
-// accepted values.  The upper bounds keep the strip arithmetic of the launchers inside int.
+// One row per option: the option name (the environment variable is MB200_ + its upper-case form unless the row names
+// another), the default, the accepted values and how a value is read.  The upper bounds keep the strip arithmetic of
+// the launchers inside int.
 constexpr int kKnobMax = 1 << 20;
+enum KnobKind {
+  kInteger,     // a decimal int inside the accepted values
+  kSwitch,      // on for any value other than 0; in the environment, for any non-empty value not starting with '0'
+};
 struct KnobSpec {
   const char *name;
   int TuningKnobs::*field;
   int fallback;
   bool (*valid)(int);
+  KnobKind kind;
+  const char *env;
 };
+bool any_value(int) { return true; }
 const KnobSpec kKnobs[] = {
     {"mma_strip", &TuningKnobs::mma_strip, 512, [](int v) { return v >= 8 && v <= kKnobMax; }},   // rounded up to 8
     {"mma_minb", &TuningKnobs::mma_minb, 4, [](int v) { return v == 3 || v == 4; }},
     {"mma_l2pf", &TuningKnobs::mma_l2pf, -1, [](int v) { return v >= -1 && v <= 1; }},    // -1: windows of <= 9 taps
+    // matrix path of the separable convolution: -1 automatic (float in / float out passes), 0 never, 1 whenever possible
+    {"conv_mma", &TuningKnobs::conv_mma, -1, [](int v) { return v >= -1 && v <= 1; }, kInteger, "MB200_MMA"},
     {"pair", &TuningKnobs::pair, 1, [](int v) { return v == 0 || v == 1; }},
     {"pair_async", &TuningKnobs::pair_async, 1, [](int v) { return v == 0 || v == 1; }},
     {"pair_async_col", &TuningKnobs::pair_async_col, -1, [](int v) { return v >= -1 && v <= 1; }},   // -1: < 33 taps
@@ -80,8 +90,26 @@ const KnobSpec kKnobs[] = {
     {"resize_chunk", &TuningKnobs::resize_chunk, 16, [](int v) { return v == 8 || v == 16; }},
     {"resize_slots", &TuningKnobs::resize_slots, 0, [](int v) { return v == 0 || v == 2 || v == 3; }},
     {"resize_strip", &TuningKnobs::resize_strip, 0, [](int v) { return v >= 0 && v <= kKnobMax; }},  // 0: automatic
+    // switches that force the generic kernels, so that tests can compare them with the specialised ones
+    {"no_rank1", &TuningKnobs::no_rank1, 0, any_value, kSwitch},
+    {"no_morph_stream", &TuningKnobs::no_morph_stream, 0, any_value, kSwitch},
+    {"no_resize_stream", &TuningKnobs::no_resize_stream, 0, any_value, kSwitch},
+    {"no_fused_unsharp", &TuningKnobs::no_fused_unsharp, 0, any_value, kSwitch},
+    // opt-in paths that measured slower than the defaults
+    {"resize_regular_h", &TuningKnobs::resize_regular_h, 0, any_value, kSwitch},
+    {"resize_fused", &TuningKnobs::resize_fused, 0, any_value, kSwitch},
 };
 constexpr size_t kNumKnobs = sizeof(kKnobs) / sizeof(kKnobs[0]);
+
+int parse_env(const KnobSpec &k, const char *s) {
+  if (!s || !*s) return k.fallback;
+  if (k.kind == kSwitch) return *s != '0';
+  char *end = nullptr;
+  const long parsed = std::strtol(s, &end, 10);
+  if (*end == '\0' && parsed >= INT_MIN && parsed <= INT_MAX && k.valid(static_cast<int>(parsed)))
+    return static_cast<int>(parsed);
+  return k.fallback;
+}
 
 struct KnobStore {
   std::atomic<int> value[kNumKnobs];
@@ -90,15 +118,7 @@ struct KnobStore {
       char env[64] = "MB200_";
       for (size_t j = 0; kKnobs[i].name[j] && j + 7 < sizeof(env); ++j)
         env[6 + j] = static_cast<char>(std::toupper(static_cast<unsigned char>(kKnobs[i].name[j])));
-      int v = kKnobs[i].fallback;
-      const char *s = std::getenv(env);
-      if (s && *s) {
-        char *end = nullptr;
-        const long parsed = std::strtol(s, &end, 10);
-        if (*end == '\0' && parsed >= INT_MIN && parsed <= INT_MAX && kKnobs[i].valid(static_cast<int>(parsed)))
-          v = static_cast<int>(parsed);
-      }
-      value[i].store(v, std::memory_order_relaxed);
+      value[i].store(parse_env(kKnobs[i], std::getenv(kKnobs[i].env ? kKnobs[i].env : env)), std::memory_order_relaxed);
     }
   }
 };
@@ -113,9 +133,15 @@ int knob_index(const char *name) {
 }
 
 const char *const kFamilyNames[kLaunchFamilies] = {
-    "conv_pair_launches", "conv_pair_async_launches", "conv_generic_launches", "resize_v_stream_launches",
-    "resize_h_tma_launches", "resize_h_stream_launches", "resize_regular_launches", "resize_gather_launches"};
+    "conv_mma_launches", "conv_pair_launches", "conv_pair_async_launches", "conv_generic_launches",
+    "resize_v_stream_launches", "resize_h_tma_launches", "resize_h_stream_launches", "resize_regular_launches",
+    "resize_gather_launches"};
 std::atomic<unsigned long long> g_family_launches[kLaunchFamilies];
+int family_index(const char *name) {
+  for (int f = 0; f < kLaunchFamilies; ++f)
+    if (std::strcmp(kFamilyNames[f], name) == 0) return f;
+  return -1;
+}
 }  // namespace
 
 TuningKnobs tuning_knobs() {
@@ -125,31 +151,7 @@ TuningKnobs tuning_knobs() {
   return t;
 }
 
-int set_tuning_knob(const char *name, int value) {
-  const int i = knob_index(name);
-  if (i < 0) return MB200_EUNSUPPORTED;
-  if (!kKnobs[i].valid(value)) return MB200_EINVAL;
-  knob_store().value[i].store(value, std::memory_order_relaxed);
-  return MB200_OK;
-}
-
-bool get_tuning_knob(const char *name, int *value) {
-  const int i = knob_index(name);
-  if (i < 0) return false;
-  *value = knob_store().value[i].load(std::memory_order_relaxed);
-  return true;
-}
-
 void count_family(LaunchFamily family) { g_family_launches[family].fetch_add(1, std::memory_order_relaxed); }
-
-bool get_family_count(const char *name, int *value) {
-  for (int f = 0; f < kLaunchFamilies; ++f)
-    if (std::strcmp(kFamilyNames[f], name) == 0) {
-      *value = static_cast<int>(g_family_launches[f].load(std::memory_order_relaxed) & 0x7fffffff);
-      return true;
-    }
-  return false;
-}
 
 int ensure_device() {
   int dev = -1;
@@ -287,6 +289,27 @@ int mb200_set_device(int device) {
   cudaError_t e = cudaSetDevice(device);
   if (e != cudaSuccess) { cudaGetLastError(); return cuda_fail(e, "cudaSetDevice"); }
   return ensure_device();
+}
+
+// Test / developer hook: the options of kKnobs (initialised from the environment) can be changed at run time, e.g. to
+// compare a specialised kernel with the generic one in one process.  mb200_get_option also reads the launch counters.
+int mb200_set_option(const char *name, int value) {
+  if (!name) return fail(MB200_EINVAL, "set_option: null name");
+  const int i = knob_index(name);
+  if (i < 0) return fail(MB200_EINVAL, "set_option: unknown option '%s'", name);
+  const KnobSpec &k = kKnobs[i];
+  if (!k.valid(value)) return fail(MB200_EINVAL, "set_option: %d is not a valid value of '%s'", value, name);
+  knob_store().value[i].store(k.kind == kSwitch ? value != 0 : value, std::memory_order_relaxed);
+  return MB200_OK;
+}
+
+int mb200_get_option(const char *name, int *value) {
+  if (!name || !value) return fail(MB200_EINVAL, "get_option: null argument");
+  const int i = knob_index(name), f = family_index(name);
+  if (i >= 0) *value = knob_store().value[i].load(std::memory_order_relaxed);
+  else if (f >= 0) *value = static_cast<int>(g_family_launches[f].load(std::memory_order_relaxed) & 0x7fffffff);
+  else return fail(MB200_EINVAL, "get_option: unknown option '%s'", name);
+  return MB200_OK;
 }
 
 const char *mb200_last_error(void) { return t_error; }

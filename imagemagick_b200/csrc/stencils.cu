@@ -754,10 +754,6 @@ int auto_level(float *buf, size_t n, unsigned *d_range, cudaStream_t s) {
   return e == cudaSuccess ? MB200_OK : cuda_fail(e, "adaptive: auto-level launch");
 }
 
-struct KernelList {               // owns a mb200_kernel_info chain
-  mb200_kernel_info *k = nullptr;
-  ~KernelList() { if (k) mb200_destroy_kernel_info(k); }
-};
 struct DeviceTemp {
   void *p = nullptr;
   cudaStream_t s;
@@ -805,12 +801,8 @@ int launch_adaptive(const float *src, float *dst, size_t w, size_t h, int channe
     else kernels[centre] += 1.0 - normalize;
     if (sigma < kEps) kernels[centre] = 1.0;
   }
-  KernelList edge_k, blur_k;
-  edge_k.k = mb200_edge_kernel(radius);
-  blur_k.k = mb200_acquire_kernel_builtin(MB200_BlurKernel, radius, sigma, 0.0, 0.0);
-  if (!edge_k.k || !blur_k.k) return fail(MB200_ENOMEM, "adaptive: kernels");
-  blur_k.k->next = mb200_acquire_kernel_builtin(MB200_BlurKernel, radius, sigma, 90.0, 0.0);
-  if (!blur_k.k->next) return fail(MB200_ENOMEM, "adaptive: kernels");
+  const KernelList edge_k(mb200_edge_kernel(radius)), blur_k = blur_kernel_pair(radius, sigma);
+  if (!edge_k || !blur_k) return fail(MB200_ENOMEM, "adaptive: kernels");
 
   DeviceTemp edge(s), tmp(s), range(s), d_offsets(s);
   if ((rc = edge.alloc(n * sizeof(float))) || (rc = tmp.alloc(n * sizeof(float))) || (rc = range.alloc(2 * sizeof(unsigned))) ||
@@ -819,10 +811,10 @@ int launch_adaptive(const float *src, float *dst, size_t w, size_t h, int channe
   float *d_edge = static_cast<float *>(edge.p), *d_tmp = static_cast<float *>(tmp.p);
   unsigned *d_range = static_cast<unsigned *>(range.p);
   // EdgeImage -> AutoLevel -> BlurImage (row kernel, then the rotated one: float intermediate) -> AutoLevel
-  if ((rc = exact_convolve(src, d_edge, w, h, channels, edge_k.k, s))) return rc;
+  if ((rc = exact_convolve(src, d_edge, w, h, channels, edge_k.get(), s))) return rc;
   if ((rc = auto_level(d_edge, n, d_range, s))) return rc;
-  if ((rc = exact_convolve(d_edge, d_tmp, w, h, channels, blur_k.k, s))) return rc;
-  if ((rc = exact_convolve(d_tmp, d_edge, w, h, channels, blur_k.k->next, s))) return rc;
+  if ((rc = exact_convolve(d_edge, d_tmp, w, h, channels, blur_k.get(), s))) return rc;
+  if ((rc = exact_convolve(d_tmp, d_edge, w, h, channels, blur_k->next, s))) return rc;
   if ((rc = auto_level(d_edge, n, d_range, s))) return rc;
 
   double *d_kernels = nullptr;

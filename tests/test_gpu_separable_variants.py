@@ -441,6 +441,24 @@ def test_resize_strip_count_past_the_grid_limit_falls_back():
     assert max_ulp(got, want) <= 1
 
 
+def test_resize_table_cache_eviction():
+    """The axis tables are cached per (device, filter, options, in_n, out_n), at most 64 of them.  Resizes through 70
+    more keys evict the first one; coming back to it rebuilds its tables, and the streaming kernels serve it again
+    with the same bits."""
+    src = make_image(254, 198, 4, seed=21, kind="alpha_blocks")
+    want = orc_resize(src, 127, 99, im.LanczosFilter)
+    first, counts = counted(lambda: _host(im.ResizeImage(_dev(src), 127, 99, im.LanczosFilter)), RESIZE_FAMILIES)
+    assert counts["resize_v_stream_launches"] == 1, counts
+    assert max_ulp(first, want) <= 1
+    for k in range(70):                  # 70 distinct x keys (2 (64 + k) -> 64 + k), one shared y key
+        other = make_image(2 * (64 + k), 16, 4, seed=k, kind="alpha_blocks")
+        got = _host(im.ResizeImage(_dev(other), 64 + k, 8, im.LanczosFilter))
+        assert max_ulp(got, orc_resize(other, 64 + k, 8, im.LanczosFilter)) <= 1, k
+    again, counts = counted(lambda: _host(im.ResizeImage(_dev(src), 127, 99, im.LanczosFilter)), RESIZE_FAMILIES)
+    assert counts["resize_v_stream_launches"] == 1, counts
+    assert np.array_equal(again, first)
+
+
 # ---- 4. device buffers that are not 16-byte aligned -----------------------------------------------------------------
 def _unaligned(a):
     """A pixel cache whose data pointer is one float past a 16-byte boundary."""
