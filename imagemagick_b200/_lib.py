@@ -121,6 +121,12 @@ PROTOTYPES = {
     "mb200_statistic_image": (_i, [_vp, _vp, _sz, _sz, _i, _i, _sz, _sz]),
     "mb200_rotational_blur_image": (_i, [_vp, _vp, _sz, _sz, _i, _d]),
     "mb200_bilateral_blur_image": (_i, [_vp, _vp, _sz, _sz, _i, _sz, _sz, _d, _d]),
+    "mb200_despeckle_image_dev": (_i, [_vp, _vp, _sz, _sz, _i, _vp]),
+    "mb200_local_contrast_image_dev": (_i, [_vp, _vp, _sz, _sz, _i, _d, _d, _vp]),
+    "mb200_wavelet_denoise_image_dev": (_i, [_vp, _vp, _sz, _sz, _i, _d, _d, _vp]),
+    "mb200_despeckle_image": (_i, [_vp, _vp, _sz, _sz, _i]),
+    "mb200_local_contrast_image": (_i, [_vp, _vp, _sz, _sz, _i, _d, _d]),
+    "mb200_wavelet_denoise_image": (_i, [_vp, _vp, _sz, _sz, _i, _d, _d]),
     "mb200_emboss_kernel": (KernelPtr, [_d, _d]),
     "mb200_equalize_image_dev": (_i, [_vp, _sz, _sz, _i, _i, _vp]),
     "mb200_emboss_image_dev": (_i, [_vp, _vp, _sz, _sz, _i, _d, _d, _vp]),

@@ -9,6 +9,8 @@ include/magick_b200.h:
     EqualizeImage                                                   enhance.c:2040
     BilateralBlurImage, RotationalBlurImage                         effect.c:821/3129
     StatisticImage                                                  statistic.c:2918
+    DespeckleImage, LocalContrastImage                              effect.c:1308/2013
+    WaveletDenoiseImage                                             visual-effects.c:3515
     MorphologyImage, AcquireKernelInfo                              morphology.c:4129/485
     ResizeImage, SampleImage, ScaleImage, ThumbnailImage (pixel)    resize.c:3761/3907/4106/4591
     TransformImageColorspace                                        colorspace.c:1751
@@ -271,6 +273,24 @@ def SelectiveBlurImage(image: Image, radius: float, sigma: float, threshold: flo
     """MagickCore/effect.c:3406 (threshold in quantum units)."""
     return _same_size_op(image, "mb200_selective_blur_image_dev", "mb200_selective_blur_image", float(radius), float(sigma),
                          float(threshold))
+
+
+def DespeckleImage(image: Image) -> Image:
+    """MagickCore/effect.c:1308."""
+    return _same_size_op(image, "mb200_despeckle_image_dev", "mb200_despeckle_image")
+
+
+def LocalContrastImage(image: Image, radius: float, strength: float) -> Image:
+    """MagickCore/effect.c:2013 (-local-contrast RxS).  MagickB200Error (EUNSUPPORTED) where the kernel width
+    max(columns, rows) * 0.002 * |radius| exceeds columns - 1."""
+    return _same_size_op(image, "mb200_local_contrast_image_dev", "mb200_local_contrast_image", float(radius),
+                         float(strength))
+
+
+def WaveletDenoiseImage(image: Image, threshold: float, softness: float = 0.0) -> Image:
+    """MagickCore/visual-effects.c:3515 (threshold in quantum units).  MagickB200Error (EUNSUPPORTED) below 32x32."""
+    return _same_size_op(image, "mb200_wavelet_denoise_image_dev", "mb200_wavelet_denoise_image", float(threshold),
+                         float(softness))
 
 
 def MotionBlurImage(image: Image, radius: float, sigma: float, angle: float) -> Image:

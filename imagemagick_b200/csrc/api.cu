@@ -941,6 +941,67 @@ int mb200_bilateral_blur_image(const float *src, float *dst, size_t w, size_t h,
 
 }  // extern "C"
 
+// ---- DespeckleImage (effect.c:1308), LocalContrastImage (effect.c:2013), WaveletDenoiseImage (visual-effects.c:3515) -------
+extern "C" {
+
+int mb200_despeckle_image_dev(const float *src, float *dst, size_t width, size_t height, int channels, void *stream) {
+  cudaStream_t s;
+  int rc = prepare_dev(src && dst && src != dst && valid_image(width, height, channels), "despeckle", stream, &s);
+  if (rc) return rc;
+  StreamAlloc tmp(s);
+  rc = tmp.alloc(image_bytes(width, height, channels));
+  if (rc) return rc;
+  return launch_despeckle(src, dst, static_cast<float *>(tmp.ptr), width, height, channels, s);
+}
+
+int mb200_local_contrast_image_dev(const float *src, float *dst, size_t width, size_t height, int channels, double radius,
+                                   double strength, void *stream) {
+  cudaStream_t s;
+  int rc = prepare_dev(src && dst && src != dst && valid_image(width, height, channels), "local contrast", stream, &s);
+  if (!rc) rc = local_contrast_supported(width, height, radius);
+  if (rc) return rc;
+  StreamAlloc planes(s);
+  rc = planes.alloc(2 * image_bytes(width, height, 1));
+  if (rc) return rc;
+  float *luma = static_cast<float *>(planes.ptr);
+  return launch_local_contrast(src, dst, luma, luma + width * height, width, height, channels, radius, strength, s);
+}
+
+int mb200_wavelet_denoise_image_dev(const float *src, float *dst, size_t width, size_t height, int channels,
+                                    double threshold, double softness, void *stream) {
+  cudaStream_t s;
+  int rc = prepare_dev(src && dst && src != dst && valid_image(width, height, channels), "wavelet denoise", stream, &s);
+  if (!rc) rc = wavelet_denoise_supported(width, height);
+  if (rc) return rc;
+  StreamAlloc planes(s);
+  rc = planes.alloc(3 * image_bytes(width, height, channels >= 3 ? 3 : 1));
+  if (rc) return rc;
+  return launch_wavelet_denoise(src, dst, static_cast<float *>(planes.ptr), width, height, channels, threshold, softness, s);
+}
+
+int mb200_despeckle_image(const float *src, float *dst, size_t w, size_t h, int ch) {
+  return with_staging("despeckle", src, w, h, ch, dst, w, h, [&](const float *s, float *d, cudaStream_t st) {
+    return mb200_despeckle_image_dev(s, d, w, h, ch, st);
+  });
+}
+
+int mb200_local_contrast_image(const float *src, float *dst, size_t w, size_t h, int ch, double radius, double strength) {
+  if (valid_image(w, h, ch) && local_contrast_supported(w, h, radius) != MB200_OK) return MB200_EUNSUPPORTED;  // no staging
+  return with_staging("local contrast", src, w, h, ch, dst, w, h, [&](const float *s, float *d, cudaStream_t st) {
+    return mb200_local_contrast_image_dev(s, d, w, h, ch, radius, strength, st);
+  });
+}
+
+int mb200_wavelet_denoise_image(const float *src, float *dst, size_t w, size_t h, int ch, double threshold,
+                                double softness) {
+  if (valid_image(w, h, ch) && wavelet_denoise_supported(w, h) != MB200_OK) return MB200_EUNSUPPORTED;           // no staging
+  return with_staging("wavelet denoise", src, w, h, ch, dst, w, h, [&](const float *s, float *d, cudaStream_t st) {
+    return mb200_wavelet_denoise_image_dev(s, d, w, h, ch, threshold, softness, st);
+  });
+}
+
+}  // extern "C"
+
 // ---- ScaleImage (resize.c:4106) ---------------------------------------------------------------------------------------------
 extern "C" {
 

@@ -204,6 +204,18 @@ int launch_adaptive(const float *src, float *dst, size_t w, size_t h, int channe
 int launch_selective_blur(const float *src, float *dst, size_t w, size_t h, int channels, double radius, double sigma,
                           double threshold, void *stream);
 
+// hooks.cu: DespeckleImage (effect.c:1308), LocalContrastImage (effect.c:2013), WaveletDenoiseImage
+// (visual-effects.c:3515), bit exact.  The temporaries are the caller's: despeckle `tmp` one image; local contrast `luma`
+// and `inter` one float plane each; wavelet `planes` 3 * (channels >= 3 ? 3 : 1) float planes.  The *_supported checks
+// are the declines (MB200_EUNSUPPORTED where the reference reads memory it never wrote), run before anything is allocated.
+int launch_despeckle(const float *src, float *dst, float *tmp, size_t w, size_t h, int channels, void *stream);
+int local_contrast_supported(size_t w, size_t h, double radius);
+int launch_local_contrast(const float *src, float *dst, float *luma, float *inter, size_t w, size_t h, int channels,
+                          double radius, double strength, void *stream);
+int wavelet_denoise_supported(size_t w, size_t h);
+int launch_wavelet_denoise(const float *src, float *dst, float *planes, size_t w, size_t h, int channels, double threshold,
+                           double softness, void *stream);
+
 // ScaleImage (resize.c:4106): CSR contribution lists of both axes (mb200_scale_contributions), bit exact
 int launch_scale(const float *src, size_t w, size_t h, int channels, float *dst, size_t ow, size_t oh, const int *d_xoff,
                  const int *d_xidx, const double *d_xwt, const int *d_yoff, const int *d_yidx, const double *d_ywt, void *stream);

@@ -7,9 +7,10 @@
           --wrap=MorphologyImage,--wrap=ResizeImage,--wrap=TransformImageColorspace,\
           --wrap=BilevelImage,--wrap=BlackThresholdImage,--wrap=WhiteThresholdImage,--wrap=ClampImage,\
           --wrap=SharpenImage,--wrap=EdgeImage,--wrap=SampleImage,--wrap=ThumbnailImage,--wrap=MinifyImage,--wrap=ResampleImage,--wrap=MotionBlurImage,\
-          --wrap=EmbossImage,--wrap=EqualizeImage,--wrap=StatisticImage,--wrap=RotationalBlurImage,--wrap=BilateralBlurImage,--wrap=ScaleImage,--wrap=SelectiveBlurImage,--wrap=AdaptiveBlurImage,--wrap=AdaptiveSharpenImage
+          --wrap=EmbossImage,--wrap=EqualizeImage,--wrap=StatisticImage,--wrap=RotationalBlurImage,--wrap=BilateralBlurImage,--wrap=ScaleImage,--wrap=SelectiveBlurImage,--wrap=AdaptiveBlurImage,--wrap=AdaptiveSharpenImage,\
+          --wrap=DespeckleImage,--wrap=LocalContrastImage,--wrap=WaveletDenoiseImage
   and every caller of those exported functions (effect.c:765/1709/1170/4256, morphology.c:4129,
-  resize.c:3761, colorspace.c:1751, threshold.c:805/927/2518/1087) reaches __wrap_X below.  Each wrapper follows the accelerate
+  resize.c:3761, colorspace.c:1751, threshold.c:805/927/2518/1087, effect.c:1308/2013, visual-effects.c:3515) reaches __wrap_X below.  Each wrapper follows the accelerate
   hook contract of effect.c:783-787 / resize.c:3818-3826: try the GPU; if the image is not
   eligible or the GPU path declines (returns NULL / MagickFalse without raising), run the stock
   CPU implementation (__real_X).  B200Accelerate*Image() are the same functions with the
@@ -136,8 +137,9 @@ static float *b200_cache_pixels(const Image *image, int channels, ExceptionInfo 
 
 typedef int (*same_size_op)(const float *, float *, size_t, size_t, int, const void *);
 
-/* src pixels -> new image through `op`; NULL == declined (caller falls back to the CPU).  allow_mask: the operator hands
-   Copy-trait channels through from its source, so a -channel selection is served by one extra point pass. */
+/* src pixels -> new image through `op`; NULL == declined (caller falls back to the CPU).  allow_mask 1: the operator hands
+   Copy-trait channels through from its source, so a -channel selection is served by one extra point pass; 2: the
+   operator ignores the selection (it computes the same channels whatever their traits), so it is served as is. */
 static Image *run_same_size_masked(const Image *image, same_size_op op, const void *args, int allow_mask,
                                    ExceptionInfo *exception)
 {
@@ -157,7 +159,7 @@ static Image *run_same_size_masked(const Image *image, same_size_op op, const vo
       q = GetAuthenticPixels(out, 0, 0, out->columns, out->rows, attempt);
       if (q == (Quantum *) NULL || b200_cache_pixels(out, ch, attempt) != (float *) q ||
           op(p, (float *) q, image->columns, image->rows, ch, args) != MB200_OK ||
-          ((update_mask & ((1u << ch) - 1u)) != ((1u << ch) - 1u) &&
+          (allow_mask == 1 && (update_mask & ((1u << ch) - 1u)) != ((1u << ch) - 1u) &&
            mb200_restore_channels((float *) q, p, image->columns, image->rows, ch, update_mask) != MB200_OK) ||
           SyncAuthenticPixels(out, attempt) == MagickFalse)
         out = DestroyImage(out);
@@ -733,6 +735,41 @@ Image *B200AccelerateSelectiveBlurImage(const Image *image, const double radius,
   return run_same_size_masked(image, op_selective, &a, 1, exception);
 }
 
+/* ---- DespeckleImage (effect.c:1308), LocalContrastImage (effect.c:2013), WaveletDenoiseImage (visual-effects.c:3515) -----
+   Despeckle skips Copy-trait channels (:1412) and LocalContrast updates only R, G, B with the Update trait (:2249-2260):
+   both leave unselected channels as the source has them, so a -channel selection is served with the restore pass.
+   WaveletDenoise tests only for an Undefined trait (visual-effects.c:3607-3614): it denoises R, G and B whatever the
+   selection, and so does the GPU path. */
+typedef struct { double a, b; } hook_args;
+static int op_despeckle(const float *s, float *d, size_t w, size_t h, int ch, const void *a)
+{ (void) a; return mb200_despeckle_image(s, d, w, h, ch); }
+static int op_local_contrast(const float *s, float *d, size_t w, size_t h, int ch, const void *a)
+{ const hook_args *t = (const hook_args *) a; return mb200_local_contrast_image(s, d, w, h, ch, t->a, t->b); }
+static int op_wavelet_denoise(const float *s, float *d, size_t w, size_t h, int ch, const void *a)
+{ const hook_args *t = (const hook_args *) a; return mb200_wavelet_denoise_image(s, d, w, h, ch, t->a, t->b); }
+
+Image *B200AccelerateDespeckleImage(const Image *image, ExceptionInfo *exception)
+{ return run_same_size_masked(image, op_despeckle, (const void *) NULL, 1, exception); }
+
+Image *B200AccelerateLocalContrastImage(const Image *image, const double radius, const double strength,
+                                        ExceptionInfo *exception)
+{
+  hook_args a;
+  a.a = radius; a.b = strength;
+  return run_same_size_masked(image, op_local_contrast, &a, 1, exception);
+}
+
+/* accelerate-private.h:48 declares AccelerateWaveletDenoiseImage(image, threshold, exception): the softness argument of
+   WaveletDenoiseImage does not reach the hook, so a build that patched the #if OPENCL call site with it would denoise
+   every image with softness 0.  This hook takes softness, so a call site passes the caller's value through. */
+Image *B200AccelerateWaveletDenoiseImage(const Image *image, const double threshold, const double softness,
+                                         ExceptionInfo *exception)
+{
+  hook_args a;
+  a.a = threshold; a.b = softness;
+  return run_same_size_masked(image, op_wavelet_denoise, &a, 2, exception);
+}
+
 /* ---- ld --wrap entry points ------------------------------------------------------------------------------ */
 extern Image *__real_BlurImage(const Image *, const double, const double, ExceptionInfo *);
 extern Image *__real_GaussianBlurImage(const Image *, const double, const double, ExceptionInfo *);
@@ -881,6 +918,29 @@ Image *__wrap_BilateralBlurImage(const Image *image, const size_t width, const s
 {
   TRY(B200AccelerateBilateralBlurImage(image, width, height, intensity_sigma, spatial_sigma, exception));
   return __real_BilateralBlurImage(image, width, height, intensity_sigma, spatial_sigma, exception);
+}
+
+extern Image *__real_DespeckleImage(const Image *, ExceptionInfo *);
+extern Image *__real_LocalContrastImage(const Image *, const double, const double, ExceptionInfo *);
+extern Image *__real_WaveletDenoiseImage(const Image *, const double, const double, ExceptionInfo *);
+
+Image *__wrap_DespeckleImage(const Image *image, ExceptionInfo *exception)
+{
+  TRY(B200AccelerateDespeckleImage(image, exception));
+  return __real_DespeckleImage(image, exception);
+}
+
+Image *__wrap_LocalContrastImage(const Image *image, const double radius, const double strength, ExceptionInfo *exception)
+{
+  TRY(B200AccelerateLocalContrastImage(image, radius, strength, exception));
+  return __real_LocalContrastImage(image, radius, strength, exception);
+}
+
+Image *__wrap_WaveletDenoiseImage(const Image *image, const double threshold, const double softness,
+                                  ExceptionInfo *exception)
+{
+  TRY(B200AccelerateWaveletDenoiseImage(image, threshold, softness, exception));
+  return __real_WaveletDenoiseImage(image, threshold, softness, exception);
 }
 
 extern Image *__real_AdaptiveBlurImage(const Image *, const double, const double, ExceptionInfo *);

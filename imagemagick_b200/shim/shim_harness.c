@@ -36,6 +36,9 @@ extern Image *__real_AdaptiveSharpenImage(const Image *, const double, const dou
 extern Image *__real_SelectiveBlurImage(const Image *, const double, const double, const double, ExceptionInfo *);
 extern Image *__real_BilateralBlurImage(const Image *, const size_t, const size_t, const double, const double, ExceptionInfo *);
 extern MagickBooleanType __real_EqualizeImage(Image *, ExceptionInfo *);
+extern Image *__real_DespeckleImage(const Image *, ExceptionInfo *);
+extern Image *__real_LocalContrastImage(const Image *, const double, const double, ExceptionInfo *);
+extern Image *__real_WaveletDenoiseImage(const Image *, const double, const double, ExceptionInfo *);
 extern Image *__real_EdgeImage(const Image *, const double, ExceptionInfo *);
 extern MagickBooleanType __real_BilevelImage(Image *, const double, ExceptionInfo *);
 extern MagickBooleanType __real_BlackThresholdImage(Image *, const char *, ExceptionInfo *);
@@ -124,6 +127,12 @@ int main(void)
   CHECK("AdaptiveSharpenImage 0x1 RGB", 0, AdaptiveSharpenImage(rgb, 0.0, 1.0, ex), CPU(__real_AdaptiveSharpenImage(rgb, 0.0, 1.0, ex)));
   CHECK("SelectiveBlurImage 0x1.5 t=10% RGBA", 0, SelectiveBlurImage(rgba, 0.0, 1.5, 6553.5, ex),
         CPU(__real_SelectiveBlurImage(rgba, 0.0, 1.5, 6553.5, ex)));
+  CHECK("DespeckleImage RGBA", 0, DespeckleImage(rgba, ex), CPU(__real_DespeckleImage(rgba, ex)));
+  CHECK("DespeckleImage RGB", 0, DespeckleImage(rgb, ex), CPU(__real_DespeckleImage(rgb, ex)));
+  CHECK("LocalContrastImage 10x12.5 RGBA", 0, LocalContrastImage(rgba, 10.0, 12.5, ex), CPU(__real_LocalContrastImage(rgba, 10.0, 12.5, ex)));
+  CHECK("LocalContrastImage 40x-30 RGB", 0, LocalContrastImage(rgb, 40.0, -30.0, ex), CPU(__real_LocalContrastImage(rgb, 40.0, -30.0, ex)));
+  CHECK("WaveletDenoiseImage 10% RGBA", 0, WaveletDenoiseImage(rgba, 6553.5, 0.0, ex), CPU(__real_WaveletDenoiseImage(rgba, 6553.5, 0.0, ex)));
+  CHECK("WaveletDenoiseImage 5%+0.3 RGB", 0, WaveletDenoiseImage(rgb, 3276.75, 0.3, ex), CPU(__real_WaveletDenoiseImage(rgb, 3276.75, 0.3, ex)));
   CHECK("BilateralBlurImage 5x5 RGB", 0, BilateralBlurImage(rgb, 5, 5, 20.0, 2.0, ex), CPU(__real_BilateralBlurImage(rgb, 5, 5, 20.0, 2.0, ex)));
   k = AcquireKernelInfo("Disk:3", ex);
   CHECK("MorphologyImage Dilate Disk:3", 0, MorphologyImage(rgba, DilateMorphology, 1, k, ex), CPU(__real_MorphologyImage(rgba, DilateMorphology, 1, k, ex)));

@@ -1,5 +1,5 @@
 """Developer micro-benchmark: device-resident timings of the hot-path operators (CUDA events).
-usage: python tools/devbench.py [blur|resize|lab|dilate|gauss|conv2d|stencils|all] [size]"""
+usage: python tools/devbench.py [blur|resize|lab|dilate|gauss|conv2d|stencils|hooks|all] [size]"""
 import sys
 from pathlib import Path
 sys.path.insert(0, str(Path(__file__).resolve().parent.parent))
@@ -97,3 +97,20 @@ if which in ("stencils", "all"):
     ms = timeit(lambda: im.RotationalBlurImage(x, 5.0), iters=3); report(f"RotationalBlurImage(5) {s}^2", ms, s * s, 32)
     ms = timeit(lambda: im.MotionBlurImage(x, 0.0, 4.0, 30.0), iters=3); report(f"MotionBlurImage(0,4,30) {s}^2", ms, s * s, 32)
     ms = timeit(lambda: im.EqualizeImage(x), iters=3); report(f"EqualizeImage {s}^2", ms, s * s, 32)
+if which in ("hooks", "all"):
+    # the last three accelerate hooks at size^2 RGBA; bytes per pixel are the kernels' unique HBM traffic (DESIGN §5.7)
+    import ctypes as C
+    from imagemagick_b200 import _lib
+    x = im.Image(torch.rand(size, size, 4, device="cuda") * 65535)
+    ms = timeit(lambda: im.DespeckleImage(x), iters=3); report(f"DespeckleImage {size}^2 RGBA", ms, size * size, 128)
+    ms = timeit(lambda: im.WaveletDenoiseImage(x, 6553.5, 0.0), iters=3)
+    report(f"WaveletDenoiseImage 10% {size}^2 RGBA", ms, size * size, 240)
+    rate = C.c_double(0.0)
+    _lib.check(_lib.load().mb200_probe_fp64_fma_rate(C.byref(rate)))
+    width = int(size * 0.002 * 10.0)
+    fmas = 2 * (2 * width - 1) * size * size
+    ms = timeit(lambda: im.LocalContrastImage(x, 10.0, 12.5), iters=3)
+    print(f"{'LocalContrastImage 10x12.5 ' + str(size) + '^2 RGBA':34s} {ms:9.3f} ms  {fmas / 1e9:.1f} G DFMA  "
+          f"{fmas / (ms * 1e-3) / 1e12:.2f} T DFMA/s  {fmas / (ms * 1e-3) / rate.value * 100:5.1f}% of the probed "
+          f"{rate.value / 1e12:.2f} T DFMA/s", flush=True)
+    del x
