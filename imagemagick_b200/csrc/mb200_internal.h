@@ -28,6 +28,7 @@ struct TuningKnobs {
   int resize_tma, resize_chunk, resize_slots, resize_strip;           // resize_stream.cu
   // switches (0 / 1) that force the generic paths, or opt in to a slower one, in api.cu
   int no_rank1, no_morph_stream, no_resize_stream, resize_regular_h, no_fused_unsharp, resize_fused;
+  int conv2d_rows;                                                     // morph2d.cu: 0 automatic, else 8 / 4 / 2
 };
 TuningKnobs tuning_knobs();
 
@@ -37,6 +38,8 @@ enum LaunchFamily {
   kConvPair, kConvPairAsync, kConvGeneric,                             // conv1d.cu
   kResizeVStream, kResizeHTma, kResizeHStream,                         // resize_stream.cu
   kResizeRegular, kResizeGather,                                       // resize.cu
+  kConv2dDenseR8, kConv2dDenseR4, kConv2dDenseR2, kMorph2d, kMinmax2d, // morph2d.cu
+  kMorphStream,                                                        // morph_stream.cu
   kLaunchFamilies
 };
 void count_family(LaunchFamily family);

@@ -211,7 +211,9 @@ __global__ void __launch_bounds__(kTileW *kTileH) morph2d_kernel(const Morph2dAr
 
 // Erode / dilate, tight version: CTA = 32x8 threads, each thread produces 4 output rows (y, y+8,
 // y+16, y+24) of one column, so every active-cell offset (one broadcast LDS) is amortised over four
-// LDS.128 + min/max groups.  fminf/fmaxf compile to FMNMX(3); a NaN sample never replaces the value.
+// LDS.128 + min/max groups.  fminf/fmaxf compile to FMNMX(3); a NaN sample never replaces the value, and
+// erode keeps a NaN centre (the reference's `sample < pixel` never replaces it, morphology.c:2911) by
+// selecting it at the output stage.  RGBA stages and stores whole float4 pixels: 16-byte aligned buffers only.
 constexpr int kMmTile = 32, kMmRows = 4;
 constexpr int kMmPitch = 64;          // fixed shared-memory pitch in pixels (kernel width <= 33)
 
@@ -293,6 +295,11 @@ __global__ void __launch_bounds__(256, 4) minmax2d_kernel(const Morph2dArgs a) {
     for (int r = 0; r < kMmRows; ++r) {
       const int y = by + threadIdx.y + 8 * r;
       if (y < a.height) {
+        if (!DILATE) {
+#pragma unroll
+          for (int c = 0; c < CH; ++c)
+            if (ctr[r][c] != ctr[r][c]) acc[r][c] = ctr[r][c];
+        }
         float *o = a.dst + (static_cast<size_t>(y) * a.width + x) * CH;
         if (CH == 4) *reinterpret_cast<float4 *>(o) = make_float4(acc[r][0], acc[r][1], acc[r][2], acc[r][CH - 1]);
         else {
@@ -474,15 +481,18 @@ int launch_morph2d(const float *src, float *dst, size_t width, size_t height, in
       host[n].du = static_cast<short>(u); host[n].dv = static_cast<short>(v); host[n].pad = 0.f; host[n].k = kept;
       ++n;
     }
-  if (method == MB200_ConvolveMorphology && n == total &&
-      ((reinterpret_cast<uintptr_t>(src) | reinterpret_cast<uintptr_t>(dst)) & 15) == 0) {
-    // every cell is part of the neighbourhood: register-tiled dense kernel (R = 4 output rows per thread, or 2 when the
-    // staged tile of doubles would not fit)
+  const bool aligned = ((reinterpret_cast<uintptr_t>(src) | reinterpret_cast<uintptr_t>(dst)) & 15) == 0;
+  if (method == MB200_ConvolveMorphology && n == total && aligned) {
+    // every cell is part of the neighbourhood: register-tiled dense kernel (R = 8 or 4 output rows per thread while the
+    // staged tile of doubles leaves room for two CTAs per SM, else 2 while it fits at all).  The conv2d_rows option
+    // forces an R whose tile fits.
     free(host);
     auto tile_bytes = [&](int R) {
       return (static_cast<size_t>((total + 1) & ~1) + static_cast<size_t>(32 + kw - 1) * (8 * R + kh - 1) * channels) * sizeof(double);
     };
-    const int R = tile_bytes(8) <= 110 * 1024 ? 8 : tile_bytes(4) <= 110 * 1024 ? 4 : (tile_bytes(2) <= 200 * 1024 ? 2 : 0);
+    const int forced = tuning_knobs().conv2d_rows;
+    int R = tile_bytes(8) <= 110 * 1024 ? 8 : tile_bytes(4) <= 110 * 1024 ? 4 : (tile_bytes(2) <= 200 * 1024 ? 2 : 0);
+    if (forced != 0 && tile_bytes(forced) <= 200 * 1024) R = forced;
     if (R != 0) {
       double *d_taps = nullptr;
       cudaError_t e = cudaMallocAsync(reinterpret_cast<void **>(&d_taps), sizeof(double) * static_cast<size_t>(total), temp_pool(), s);
@@ -517,6 +527,7 @@ int launch_morph2d(const float *src, float *dst, size_t width, size_t height, in
       }
 #undef MB200_DENSE
       count_launch();
+      count_family(R == 8 ? kConv2dDenseR8 : R == 4 ? kConv2dDenseR4 : kConv2dDenseR2);
       e = cudaGetLastError();
       cudaFreeAsync(d_taps, s);
       if (e != cudaSuccess) return cuda_fail(e, "conv2d launch");
@@ -545,7 +556,8 @@ int launch_morph2d(const float *src, float *dst, size_t width, size_t height, in
   a.ox = ox; a.oy = oy; a.kw = kw; a.kh = kh; a.ncells = n;
   a.cells = static_cast<const Cell *>(d_cells);
   a.bias = bias; a.gamma_scale = gamma_scale; a.method = method; a.changed = d_changed;
-  if ((method == MB200_ErodeMorphology || method == MB200_DilateMorphology) && n <= 1024 && kw <= kMmPitch - kMmTile + 1) {
+  if ((method == MB200_ErodeMorphology || method == MB200_DilateMorphology) && n <= 1024 && kw <= kMmPitch - kMmTile + 1 &&
+      (channels != 4 || aligned)) {         // RGBA moves float4 pixels: unaligned buffers take morph2d_kernel below
     const int th = kMmTile + kh - 1;
     const size_t msmem = static_cast<size_t>(kMmPitch) * th * channels * sizeof(float);
     if (msmem <= 160 * 1024) {
@@ -569,6 +581,7 @@ int launch_morph2d(const float *src, float *dst, size_t width, size_t height, in
       }
 #undef MB200_MM
       count_launch();
+      count_family(kMinmax2d);
       e = cudaGetLastError();
       cudaFreeAsync(d_cells, s);
       if (e != cudaSuccess) return cuda_fail(e, "minmax2d launch");
@@ -591,6 +604,7 @@ int launch_morph2d(const float *src, float *dst, size_t width, size_t height, in
   }
 #undef MB200_LAUNCH
   count_launch();
+  count_family(kMorph2d);
   e = cudaGetLastError();
   cudaFreeAsync(d_cells, s);
   if (e != cudaSuccess) return cuda_fail(e, "morph2d launch");

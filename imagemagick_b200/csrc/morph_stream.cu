@@ -90,6 +90,11 @@ __global__ void __launch_bounds__(128) minmax_stream_kernel(const StreamArgs a) 
   const float *col = a.src + static_cast<size_t>(xc) * CH;
   float *outp = a.dst + static_cast<size_t>(y0) * pitch + static_cast<size_t>(max(x, 0)) * CH;
   const float init = DILATE ? 0.0f : __int_as_float(0x7f800000);
+  // Erode keeps a NaN centre (the reference's `sample < pixel` never replaces it, morphology.c:2911), which the min
+  // fold drops: bit q of centre_nan records that accumulator q's centre sample -- the lane's own sample at kernel row
+  // oy, slot (s + cbase) mod K -- has a NaN component, and its output then takes the centre's NaN components.
+  const int cbase = K - 1 - a.oy;                                // 0 <= oy < K
+  unsigned centre_nan = 0;
 
   Px<CH> acc[K], pre[K];
 #pragma unroll
@@ -110,6 +115,13 @@ __global__ void __launch_bounds__(128) minmax_stream_kernel(const StreamArgs a) 
       const Px<CH> p = pre[s];
       pre[s] = load_px<CH>(col + static_cast<size_t>(min(max(r, 0), hmax)) * pitch);
       ++r;
+      if constexpr (!DILATE) {
+        unsigned nan = 0;
+#pragma unroll
+        for (int c = 0; c < CH; ++c) nan |= (__float_as_uint(p.v[c]) & 0x7fffffffu) > 0x7f800000u;
+        const int cs = s + cbase >= K ? s + cbase - K : s + cbase;
+        centre_nan |= nan << cs;
+      }
       Px<CH> h[R + 1];
       h[0] = p;
 #pragma unroll
@@ -131,7 +143,18 @@ __global__ void __launch_bounds__(128) minmax_stream_kernel(const StreamArgs a) 
         }
       }
       const int done = s % K;
-      if (writer && static_cast<unsigned>(j) < static_cast<unsigned>(nout)) store_px<CH>(outp, acc[done]);
+      if (writer && static_cast<unsigned>(j) < static_cast<unsigned>(nout)) {
+        if constexpr (!DILATE) {
+          if ((centre_nan >> done) & 1u) {             // rare: reload the centre (this output's own source pixel)
+            const Px<CH> ctr = load_px<CH>(col + static_cast<size_t>(y0 + j) * pitch);
+#pragma unroll
+            for (int c = 0; c < CH; ++c)
+              if (ctr.v[c] != ctr.v[c]) acc[done].v[c] = ctr.v[c];
+          }
+        }
+        store_px<CH>(outp, acc[done]);
+      }
+      if constexpr (!DILATE) centre_nan &= ~(1u << done);
 #pragma unroll
       for (int c = 0; c < CH; ++c) acc[done].v[c] = init;
       if (j >= 0) outp += pitch;
@@ -230,6 +253,7 @@ int launch_morph_stream(const float *src, float *dst, size_t width, size_t heigh
   if (grid.y > 65535) return MB200_EUNSUPPORTED;
   const cudaError_t e = entry->fn[channels == 4 ? 1 : 0][dilate ? 1 : 0](a, grid, static_cast<cudaStream_t>(stream));
   count_launch();
+  count_family(kMorphStream);
   if (e != cudaSuccess) return cuda_fail(e, "morph_stream launch");
   return MB200_OK;
 }

@@ -90,6 +90,8 @@ const KnobSpec kKnobs[] = {
     {"resize_chunk", &TuningKnobs::resize_chunk, 16, [](int v) { return v == 8 || v == 16; }},
     {"resize_slots", &TuningKnobs::resize_slots, 0, [](int v) { return v == 0 || v == 2 || v == 3; }},
     {"resize_strip", &TuningKnobs::resize_strip, 0, [](int v) { return v >= 0 && v <= kKnobMax; }},  // 0: automatic
+    // output rows per thread of the dense 2-D convolution: 0 automatic, 8 / 4 / 2 forced where that tile fits
+    {"conv2d_rows", &TuningKnobs::conv2d_rows, 0, [](int v) { return v == 0 || v == 2 || v == 4 || v == 8; }},
     // switches that force the generic kernels, so that tests can compare them with the specialised ones
     {"no_rank1", &TuningKnobs::no_rank1, 0, any_value, kSwitch},
     {"no_morph_stream", &TuningKnobs::no_morph_stream, 0, any_value, kSwitch},
@@ -135,7 +137,8 @@ int knob_index(const char *name) {
 const char *const kFamilyNames[kLaunchFamilies] = {
     "conv_mma_launches", "conv_pair_launches", "conv_pair_async_launches", "conv_generic_launches",
     "resize_v_stream_launches", "resize_h_tma_launches", "resize_h_stream_launches", "resize_regular_launches",
-    "resize_gather_launches"};
+    "resize_gather_launches", "conv2d_dense_r8_launches", "conv2d_dense_r4_launches", "conv2d_dense_r2_launches",
+    "morph2d_launches", "minmax2d_launches", "morph_stream_launches"};
 std::atomic<unsigned long long> g_family_launches[kLaunchFamilies];
 int family_index(const char *name) {
   for (int f = 0; f < kLaunchFamilies; ++f)

@@ -364,12 +364,14 @@ KNOB_RANGES = {
     "resize_slots": ([0, 2, 3], [1, 4, -1]),
     "resize_strip": ([0, 7, 24], [-1]),
     "conv_mma": ([-1, 0, 1], [-2, 2]),
+    "conv2d_rows": ([0, 2, 4, 8], [-1, 1, 3, 6, 16]),
 }
 SWITCHES = ["no_rank1", "no_morph_stream", "no_resize_stream", "resize_regular_h", "no_fused_unsharp", "resize_fused"]
 KNOB_RANGES.update({name: ([0, 1], []) for name in SWITCHES})      # a switch takes any int (see the test below)
 COUNTERS = ["conv_mma_launches", "conv_pair_launches", "conv_pair_async_launches", "conv_generic_launches",
             "resize_v_stream_launches", "resize_h_tma_launches", "resize_h_stream_launches", "resize_regular_launches",
-            "resize_gather_launches"]
+            "resize_gather_launches", "conv2d_dense_r8_launches", "conv2d_dense_r4_launches", "conv2d_dense_r2_launches",
+            "morph2d_launches", "minmax2d_launches", "morph_stream_launches"]
 
 
 @pytest.mark.parametrize("name", sorted(KNOB_RANGES))
@@ -415,15 +417,15 @@ def test_invalid_environment_values_fall_back_to_the_defaults():
     env = dict(os.environ, MB200_MMA_STRIP="0", MB200_COL_ROT="0", MB200_ROW_PAIR_ROT="-3", MB200_MMA_MINB="7",
                MB200_RESIZE_CHUNK="12", MB200_RESIZE_SLOTS="1", MB200_RESIZE_TMA="x", MB200_ROW_ROT="5",
                MB200_RESIZE_STRIP="24", MB200_PAIR_ASYNC_COL="0", MB200_NO_RANK1="yes", MB200_NO_MORPH_STREAM="0",
-               MB200_MMA="abc")
+               MB200_MMA="abc", MB200_CONV2D_ROWS="3")
     code = ("import ctypes as C\nfrom imagemagick_b200 import _lib\nv = C.c_int()\n"
             "for n in %r:\n    assert _lib.load().mb200_get_option(n.encode(), C.byref(v)) == 0\n"
             "    print(n, v.value)\n" % [
                 "mma_strip", "col_rot", "row_pair_rot", "mma_minb", "resize_chunk", "resize_slots", "resize_tma",
-                "row_rot", "resize_strip", "pair_async_col", "no_rank1", "no_morph_stream", "conv_mma"])
+                "row_rot", "resize_strip", "pair_async_col", "no_rank1", "no_morph_stream", "conv_mma", "conv2d_rows"])
     p = subprocess.run([sys.executable, "-c", code], env=env, cwd=str(ROOT), capture_output=True, text=True, timeout=120)
     assert p.returncode == 0, p.stderr
     got = dict(line.split() for line in p.stdout.split("\n") if line)
     assert got == {"mma_strip": "512", "col_rot": "16", "row_pair_rot": "16", "mma_minb": "4", "resize_chunk": "16",
                    "resize_slots": "0", "resize_tma": "1", "row_rot": "5", "resize_strip": "24", "pair_async_col": "0",
-                   "no_rank1": "1", "no_morph_stream": "0", "conv_mma": "-1"}
+                   "no_rank1": "1", "no_morph_stream": "0", "conv_mma": "-1", "conv2d_rows": "0"}

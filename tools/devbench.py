@@ -1,5 +1,5 @@
 """Developer micro-benchmark: device-resident timings of the hot-path operators (CUDA events).
-usage: python tools/devbench.py [blur|resize|lab|dilate|gauss|conv2d|stencils|hooks|all] [size]"""
+usage: python tools/devbench.py [blur|resize|lab|dilate|erode|gauss|conv2d|stencils|hooks|all] [size]"""
 import sys
 from pathlib import Path
 sys.path.insert(0, str(Path(__file__).resolve().parent.parent))
@@ -71,6 +71,11 @@ if which in ("dilate", "all"):
     x = im.Image(torch.rand(size, size, 4, device="cuda") * 65535)
     k = im.AcquireKernelInfo("Disk:3")
     ms = timeit(lambda: im.MorphologyImage(x, im.DilateMorphology, 1, k)); report(f"Dilate Disk:3 {size}^2", ms, size * size, 32)
+    del x
+if which in ("erode", "all"):
+    x = im.Image(torch.rand(size, size, 4, device="cuda") * 65535)
+    k = im.AcquireKernelInfo("Disk:3")
+    ms = timeit(lambda: im.MorphologyImage(x, im.ErodeMorphology, 1, k)); report(f"Erode Disk:3 {size}^2", ms, size * size, 32)
     del x
 if which in ("gauss", "all"):
     s = min(size, 4096)
