@@ -154,6 +154,14 @@ PROTOTYPES = {
     "mb200_black_threshold_image": (_i, [_vp, _sz, _sz, _i, _i, C.c_char_p]),
     "mb200_white_threshold_image": (_i, [_vp, _sz, _sz, _i, _i, C.c_char_p]),
     "mb200_clamp_image": (_i, [_vp, _sz, _sz, _i]),
+    "mb200_contrast_image_dev": (_i, [_vp, _sz, _sz, _i, _i, _vp]),
+    "mb200_modulate_image_dev": (_i, [_vp, _sz, _sz, _i, _d, _d, _d, _i, _i, _vp]),
+    "mb200_grayscale_image_dev": (_i, [_vp, _sz, _sz, _i, _i, _i, _vp]),
+    "mb200_function_image_dev": (_i, [_vp, _sz, _sz, _i, _i, _sz, C.POINTER(_d), C.c_uint, _vp]),
+    "mb200_contrast_image": (_i, [_vp, _sz, _sz, _i, _i]),
+    "mb200_modulate_image": (_i, [_vp, _sz, _sz, _i, _d, _d, _d, _i, _i]),
+    "mb200_grayscale_image": (_i, [_vp, _sz, _sz, _i, _i, _i]),
+    "mb200_function_image": (_i, [_vp, _sz, _sz, _i, _i, _sz, C.POINTER(_d), C.c_uint]),
 }
 
 _lib = None

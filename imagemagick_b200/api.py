@@ -15,6 +15,8 @@ include/magick_b200.h:
     ResizeImage, SampleImage, ScaleImage, ThumbnailImage (pixel)    resize.c:3761/3907/4106/4591
     TransformImageColorspace                                        colorspace.c:1751
     BilevelImage, BlackThresholdImage, WhiteThresholdImage, ClampImage  threshold.c:805/927/2518/1087
+    ContrastImage, ModulateImage, GrayscaleImage                    enhance.c:1370/3461/2474
+    FunctionImage                                                   statistic.c:1064
 
 An `Image` wraps the pixel cache: an (rows, columns, channels) float32 array of raw
 Quantum values (0..65535), either a NumPy array (host; every call stages through
@@ -22,8 +24,8 @@ HBM and back -- the end-to-end path) or a CUDA torch tensor (device-resident; th
 kernels run on torch's current stream and the result stays in HBM).
 
 Operators that return `Image *` in the reference return a NEW Image here and never
-modify their input; TransformImageColorspace works in place and returns True, like
-the reference.  Failures raise MagickB200Error (the reference returns NULL / MagickFalse
+modify their input; TransformImageColorspace, the threshold operators, Contrast, Modulate,
+Grayscale and Function work in place and return True, like the reference.  Failures raise MagickB200Error (the reference returns NULL / MagickFalse
 and fills an ExceptionInfo); MB200_EUNSUPPORTED is the "decline" signal on which the
 MagickCore shim falls back to the stock CPU path.  Nothing here computes pixels on
 the CPU.
@@ -62,6 +64,15 @@ LCHColorspace, LCHabColorspace, LCHuvColorspace, OklabColorspace, OklchColorspac
 LogColorspace, YCCColorspace = 15, 28
 LMSColorspace, LuvColorspace, xyYColorspace, DisplayP3Colorspace, Adobe98Colorspace, ProPhotoColorspace, CAT02LMSColorspace = 16, 17, 25, 35, 36, 37, 40
 HCLColorspace, HCLpColorspace, HSBColorspace, HSIColorspace, HSLColorspace, HSVColorspace, HWBColorspace = 4, 5, 6, 7, 8, 9, 10
+GRAYColorspace, LinearGRAYColorspace = 3, 33
+
+# MagickCore/pixel.h:110-120
+(UndefinedPixelIntensityMethod, AveragePixelIntensityMethod, BrightnessPixelIntensityMethod, LightnessPixelIntensityMethod,
+ MSPixelIntensityMethod, Rec601LumaPixelIntensityMethod, Rec601LuminancePixelIntensityMethod, Rec709LumaPixelIntensityMethod,
+ Rec709LuminancePixelIntensityMethod, RMSPixelIntensityMethod) = range(10)
+
+# MagickCore/statistic.h:130-137
+UndefinedFunction, ArcsinFunction, ArctanFunction, PolynomialFunction, SinusoidFunction = range(5)
 
 # kernel types of include/magick_b200.h
 (UserDefinedKernel, BlurKernel, GaussianKernel, DiskKernel, SquareKernel, DiamondKernel, OctagonKernel,
@@ -475,6 +486,75 @@ def WhiteThresholdImage(image: Image, thresholds: str) -> bool:
 def ClampImage(image: Image) -> bool:
     """MagickCore/threshold.c:1087 -- in place."""
     return _in_place(image, "mb200_clamp_image_dev", "mb200_clamp_image")
+
+
+def ContrastImage(image: Image, sharpen: bool) -> bool:
+    """MagickCore/enhance.c:1370 -- in place; alpha untouched."""
+    return _in_place(image, "mb200_contrast_image_dev", "mb200_contrast_image", 1 if sharpen else 0)
+
+
+# ParseCommandOption(MagickColorspaceOptions, ...) for the spaces ModulateImage distinguishes (enhance.c:3837-3887)
+_MODULATE_SPACES = {"hcl": HCLColorspace, "hclp": HCLpColorspace, "hsb": HSBColorspace, "hsi": HSIColorspace,
+                    "hsl": HSLColorspace, "hsv": HSVColorspace, "hwb": HWBColorspace, "lch": LCHColorspace,
+                    "lchab": LCHabColorspace, "lchuv": LCHuvColorspace}
+# IssRGBCompatibleColorspace (colorspace-private.h:1763): sRGB, RGB, scRGB, Transparent, GRAY, LinearGRAY and the wide-gamut RGBs
+_SRGB_COMPATIBLE = {sRGBColorspace, RGBColorspace, 22, 24, GRAYColorspace, LinearGRAYColorspace, Adobe98Colorspace,
+                    ProPhotoColorspace, DisplayP3Colorspace}
+
+
+def _modulate_percentages(modulate: str):
+    """The "B[,S[,H]]" geometry of -modulate (ParseGeometry's rho / sigma / xi): 1-3 numbers; the first separator may be
+    'x' (rho x sigma), the second is ','."""
+    parts = str(modulate).strip().split(",")
+    parts = parts[0].split("x", 1) + parts[1:]
+    try:
+        values = [float(p) for p in parts]
+    except ValueError:
+        values = []
+    if not 1 <= len(values) <= 3:
+        raise MagickB200Error(_lib.EINVAL, f"modulate: '{modulate}' is not of the form B[,S[,H]]")
+    return (values + [100.0, 100.0])[:3]
+
+
+def ModulateImage(image: Image, modulate: str, artifacts=None) -> bool:
+    """MagickCore/enhance.c:3461 -- in place.  `artifacts`: the image's "modulate:colorspace" (HSL unless one of HCL, HCLp,
+    HSB, HSI, HSL, HSV, HWB, LCH, LCHab, LCHuv) and "color:illuminant" (for the LCH spaces; an unparsable one selects HSL,
+    :3694-3709).  An image whose colourspace is not sRGB-compatible is re-tagged sRGB first, its pixels unchanged (:3681)."""
+    brightness, saturation, hue = _modulate_percentages(modulate)
+    artifacts = artifacts or {}
+    space = _MODULATE_SPACES.get(str(artifacts.get("modulate:colorspace", "")).strip().lower(), HSLColorspace)
+    illuminant = 5
+    if "color:illuminant" in artifacts:
+        name = str(artifacts["color:illuminant"]).strip().lower()
+        illuminant = 5 if name == "undefined" else _ILLUMINANTS.get(name, -1)
+        if illuminant < 0:
+            illuminant, space = 5, HSLColorspace
+    if image.colorspace not in _SRGB_COMPATIBLE:
+        image.colorspace = sRGBColorspace
+    return _in_place(image, "mb200_modulate_image_dev", "mb200_modulate_image", brightness, saturation, hue, space,
+                     illuminant)
+
+
+def GrayscaleImage(image: Image, method: int) -> bool:
+    """MagickCore/enhance.c:2474 -- in place.  The pixel cache is re-laid out to the gray channel (plus alpha) and the
+    image re-tagged GRAY, or LinearGRAY for the Luminance methods, as the reference's hook branch does (:2503-2511)."""
+    _in_place(image, "mb200_grayscale_image_dev", "mb200_grayscale_image", int(method), int(image.colorspace))
+    keep = [0, image.channels - 1] if image.channels in (2, 4) else [0]
+    if image.channels > len(keep):
+        pixels = image.pixels[:, :, keep]
+        image.pixels = pixels.contiguous() if image.on_device else np.ascontiguousarray(pixels)
+    luminance = method in (Rec601LuminancePixelIntensityMethod, Rec709LuminancePixelIntensityMethod)
+    image.colorspace = LinearGRAYColorspace if luminance else GRAYColorspace
+    return True
+
+
+def FunctionImage(image: Image, function: int, parameters, channels: Optional[int] = None) -> bool:
+    """MagickCore/statistic.c:1064 -- in place on the channels with the Update trait: all of them, alpha included, unless
+    `channels` (bit c = channel c, a `-channel` selection) says otherwise.  At most 32 parameters."""
+    params = [float(p) for p in parameters]
+    arr = (C.c_double * max(1, len(params)))(*params)
+    mask = (1 << image.channels) - 1 if channels is None else int(channels)
+    return _in_place(image, "mb200_function_image_dev", "mb200_function_image", int(function), len(params), arr, mask)
 
 
 def MorphologyPrimitive(image: Image, method: int, kernel: Union[str, KernelInfo], bias: float = 0.0):

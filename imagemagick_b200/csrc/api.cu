@@ -1137,3 +1137,97 @@ int mb200_motion_blur_image(const float *src, float *dst, size_t w, size_t h, in
 }
 
 }  // extern "C"
+
+// ---- ContrastImage / ModulateImage / GrayscaleImage / FunctionImage (enhance.c, statistic.c), in place ----------------
+namespace {
+int check_modulate(int illuminant) {
+  if (illuminant < MB200_AIlluminant || illuminant > MB200_F11Illuminant)
+    return fail(MB200_EINVAL, "modulate: illuminant %d is not an IlluminantType", illuminant);
+  return MB200_OK;
+}
+int check_grayscale(int method) {
+  if (method < MB200_UndefinedPixelIntensityMethod || method > MB200_RMSPixelIntensityMethod)
+    return fail(MB200_EINVAL, "grayscale: method %d is not a PixelIntensityMethod", method);
+  return MB200_OK;
+}
+int check_function(int function, size_t n, const double *params) {
+  if (function < MB200_UndefinedFunction || function > MB200_SinusoidFunction)
+    return fail(MB200_EINVAL, "function: %d is not a MagickFunction", function);
+  if (n > 0 && params == nullptr) return fail(MB200_EINVAL, "function: parameters == NULL");
+  if (n > MB200_MAX_FUNCTION_PARAMETERS)
+    return fail(MB200_EUNSUPPORTED, "function: %zu parameters (at most %d)", n, MB200_MAX_FUNCTION_PARAMETERS);
+  return MB200_OK;
+}
+}  // namespace
+
+extern "C" {
+
+int mb200_contrast_image_dev(float *buf, size_t width, size_t height, int channels, int sharpen, void *stream) {
+  cudaStream_t s;
+  const int rc = prepare_dev(buf && valid_image(width, height, channels), "contrast", stream, &s);
+  if (rc) return rc;
+  return launch_contrast(buf, width * height, channels, sharpen != 0, s);
+}
+
+int mb200_modulate_image_dev(float *buf, size_t width, size_t height, int channels, double percent_brightness,
+                             double percent_saturation, double percent_hue, int colorspace, int illuminant, void *stream) {
+  cudaStream_t s;
+  int rc = prepare_dev(buf && valid_image(width, height, channels), "modulate", stream, &s);
+  if (!rc) rc = check_modulate(illuminant);
+  if (rc) return rc;
+  return launch_modulate(buf, width * height, channels, percent_brightness, percent_saturation, percent_hue, colorspace,
+                         illuminant, s);
+}
+
+int mb200_grayscale_image_dev(float *buf, size_t width, size_t height, int channels, int method, int image_colorspace,
+                              void *stream) {
+  cudaStream_t s;
+  int rc = prepare_dev(buf && valid_image(width, height, channels), "grayscale", stream, &s);
+  if (!rc) rc = check_grayscale(method);
+  if (rc) return rc;
+  return launch_grayscale(buf, width * height, channels, method, image_colorspace, s);
+}
+
+int mb200_function_image_dev(float *buf, size_t width, size_t height, int channels, int function, size_t number_parameters,
+                             const double *parameters, unsigned update_mask, void *stream) {
+  cudaStream_t s;
+  int rc = prepare_dev(buf && valid_image(width, height, channels), "function", stream, &s);
+  if (!rc) rc = check_function(function, number_parameters, parameters);
+  if (rc) return rc;
+  return launch_function(buf, width * height, channels, function, number_parameters, parameters, update_mask, s);
+}
+
+// Host forms: the argument checks run before the buffer is staged, so a refused call moves no data.
+int mb200_contrast_image(float *buf, size_t w, size_t h, int ch, int sharpen) {
+  return in_place_host("contrast", buf, w, h, ch,
+                       [&](float *d, cudaStream_t st) { return mb200_contrast_image_dev(d, w, h, ch, sharpen, st); });
+}
+
+int mb200_modulate_image(float *buf, size_t w, size_t h, int ch, double percent_brightness, double percent_saturation,
+                         double percent_hue, int colorspace, int illuminant) {
+  const int rc = check_modulate(illuminant);
+  if (rc) return rc;
+  return in_place_host("modulate", buf, w, h, ch, [&](float *d, cudaStream_t st) {
+    return mb200_modulate_image_dev(d, w, h, ch, percent_brightness, percent_saturation, percent_hue, colorspace, illuminant,
+                                    st);
+  });
+}
+
+int mb200_grayscale_image(float *buf, size_t w, size_t h, int ch, int method, int image_colorspace) {
+  const int rc = check_grayscale(method);
+  if (rc) return rc;
+  return in_place_host("grayscale", buf, w, h, ch, [&](float *d, cudaStream_t st) {
+    return mb200_grayscale_image_dev(d, w, h, ch, method, image_colorspace, st);
+  });
+}
+
+int mb200_function_image(float *buf, size_t w, size_t h, int ch, int function, size_t number_parameters,
+                         const double *parameters, unsigned update_mask) {
+  const int rc = check_function(function, number_parameters, parameters);
+  if (rc) return rc;
+  return in_place_host("function", buf, w, h, ch, [&](float *d, cudaStream_t st) {
+    return mb200_function_image_dev(d, w, h, ch, function, number_parameters, parameters, update_mask, st);
+  });
+}
+
+}  // extern "C"

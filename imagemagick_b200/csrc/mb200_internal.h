@@ -230,6 +230,15 @@ int launch_sample(const float *src, size_t w, size_t h, int channels, float *dst
 // default): one intensity-driven histogram for all channels.  Synchronises the stream (host step between the kernels).
 int launch_equalize(float *buf, size_t npixels, int channels, int sync_channels, void *stream);
 
+// enhance.cu: ContrastImage (enhance.c:1370), ModulateImage (:3461), GrayscaleImage (:2474; channel 0 only) and
+// FunctionImage (statistic.c:1064) in place, arguments already checked
+int launch_contrast(float *buf, size_t npixels, int channels, bool sharpen, void *stream);
+int launch_modulate(float *buf, size_t npixels, int channels, double percent_brightness, double percent_saturation,
+                    double percent_hue, int colorspace, int illuminant, void *stream);
+int launch_grayscale(float *buf, size_t npixels, int channels, int method, int image_colorspace, void *stream);
+int launch_function(float *buf, size_t npixels, int channels, int function, size_t n, const double *params,
+                    unsigned update_mask, void *stream);
+
 // threshold.c point operators in place; op: 0 bilevel (t[0]), 1 black, 2 white (t = r,g,b,a), 3 clamp
 int launch_threshold(float *buf, size_t npixels, int channels, int op, const double *thresholds, void *stream);
 

@@ -8,9 +8,11 @@
           --wrap=BilevelImage,--wrap=BlackThresholdImage,--wrap=WhiteThresholdImage,--wrap=ClampImage,\
           --wrap=SharpenImage,--wrap=EdgeImage,--wrap=SampleImage,--wrap=ThumbnailImage,--wrap=MinifyImage,--wrap=ResampleImage,--wrap=MotionBlurImage,\
           --wrap=EmbossImage,--wrap=EqualizeImage,--wrap=StatisticImage,--wrap=RotationalBlurImage,--wrap=BilateralBlurImage,--wrap=ScaleImage,--wrap=SelectiveBlurImage,--wrap=AdaptiveBlurImage,--wrap=AdaptiveSharpenImage,\
-          --wrap=DespeckleImage,--wrap=LocalContrastImage,--wrap=WaveletDenoiseImage
+          --wrap=DespeckleImage,--wrap=LocalContrastImage,--wrap=WaveletDenoiseImage,\
+          --wrap=ContrastImage,--wrap=ModulateImage,--wrap=GrayscaleImage,--wrap=FunctionImage
   and every caller of those exported functions (effect.c:765/1709/1170/4256, morphology.c:4129,
-  resize.c:3761, colorspace.c:1751, threshold.c:805/927/2518/1087, effect.c:1308/2013, visual-effects.c:3515) reaches __wrap_X below.  Each wrapper follows the accelerate
+  resize.c:3761, colorspace.c:1751, threshold.c:805/927/2518/1087, effect.c:1308/2013, visual-effects.c:3515,
+  enhance.c:1370/3461/2474, statistic.c:1064) reaches __wrap_X below.  Each wrapper follows the accelerate
   hook contract of effect.c:783-787 / resize.c:3818-3826: try the GPU; if the image is not
   eligible or the GPU path declines (returns NULL / MagickFalse without raising), run the stock
   CPU implementation (__real_X).  B200Accelerate*Image() are the same functions with the
@@ -23,6 +25,7 @@
 #include "MagickCore/studio.h"
 #include "MagickCore/MagickCore.h"
 #include "MagickCore/string-private.h"          /* StringToDoubleInterval (convolve:bias, morphology.c:4163) */
+#include "MagickCore/colorspace-private.h"      /* IssRGBCompatibleColorspace (ModulateImage, enhance.c:3681) */
 #include "magick_b200.h"
 #include <string.h>
 
@@ -650,6 +653,104 @@ MagickBooleanType B200AccelerateEqualizeImage(Image *image, ExceptionInfo *excep
   return ok;
 }
 
+/* ---- in-place enhance operators (the reference's hooks AccelerateContrastImage, AccelerateModulateImage,
+   AccelerateGrayscaleImage, AccelerateFunctionImage; accelerate-private.h:50-60) ----------------------------------------
+   b200_channels[_masked] declines PseudoClass, CMYK, masks and the rest: the CPU path then serves them (and the colormap
+   step of Contrast / Modulate). */
+typedef struct {
+  int op;                       /* 0 contrast, 1 modulate, 2 grayscale, 3 function */
+  int sharpen, colorspace, illuminant, method;
+  double brightness, saturation, hue;
+  MagickFunction function;
+  size_t n;
+  const double *params;
+} enhance_args;
+
+static MagickBooleanType run_enhance(Image *image, int ch, unsigned update_mask, const enhance_args *a)
+{
+  MagickBooleanType ok = MagickFalse;
+  Quantum *q;
+  int rc = MB200_EINVAL;
+  if (ch == 0 || mb200_device_count() <= 0) return MagickFalse;
+  {
+    B200_ATTEMPT_BEGIN;
+    q = GetAuthenticPixels(image, 0, 0, image->columns, image->rows, attempt);
+    if (q != (Quantum *) NULL && b200_cache_pixels(image, ch, attempt) == (float *) q)
+      switch (a->op) {
+        case 0: rc = mb200_contrast_image((float *) q, image->columns, image->rows, ch, a->sharpen); break;
+        case 1:
+          rc = mb200_modulate_image((float *) q, image->columns, image->rows, ch, a->brightness, a->saturation, a->hue,
+                                    a->colorspace, a->illuminant);
+          break;
+        case 2: rc = mb200_grayscale_image((float *) q, image->columns, image->rows, ch, a->method, a->colorspace); break;
+        default:
+          rc = mb200_function_image((float *) q, image->columns, image->rows, ch, (int) a->function, a->n, a->params,
+                                    update_mask);
+          break;
+      }
+    /* on failure nothing was written back: the CPU path starts from the same pixels */
+    if (rc == MB200_OK && SyncAuthenticPixels(image, attempt) != MagickFalse) ok = MagickTrue;
+    B200_ATTEMPT_END;
+  }
+  return ok;
+}
+
+/* ContrastImage (enhance.c:1370) sets R, G and B whatever the channel mask says; a selection still declines here */
+MagickBooleanType B200AccelerateContrastImage(Image *image, const MagickBooleanType sharpen, ExceptionInfo *exception)
+{
+  enhance_args a;
+  (void) exception;
+  (void) memset(&a, 0, sizeof(a));
+  a.op = 0; a.sharpen = sharpen != MagickFalse ? 1 : 0;
+  return run_enhance(image, b200_channels(image), 0u, &a);
+}
+
+/* ModulateImage's pixel loop (enhance.c:3800-3898) with the caller's parse: `colorspace` as ParseCommandOption gave it
+   (UndefinedColorspace after an unparsable illuminant: HSL).  The LCH spaces' reference white is the "color:illuminant"
+   artifact (:3694-3709), read here because the hook's signature does not carry it. */
+MagickBooleanType B200AccelerateModulateImage(Image *image, const double percent_brightness, const double percent_hue,
+                                              const double percent_saturation, const ColorspaceType colorspace,
+                                              ExceptionInfo *exception)
+{
+  enhance_args a;
+  const char *artifact = GetImageArtifact(image, "color:illuminant");
+  (void) exception;
+  (void) memset(&a, 0, sizeof(a));
+  a.op = 1; a.brightness = percent_brightness; a.saturation = percent_saturation; a.hue = percent_hue;
+  a.colorspace = (int) colorspace;
+  a.illuminant = (int) D65Illuminant;
+  if (artifact != (const char *) NULL) {
+    const ssize_t type = ParseCommandOption(MagickIlluminantOptions, MagickFalse, artifact);
+    a.illuminant = type < 0 ? (int) UndefinedIlluminant : (int) type;
+  }
+  return run_enhance(image, b200_channels(image), 0u, &a);
+}
+
+/* GrayscaleImage's pixel loop (enhance.c:2532-2639): the gray value into channel 0.  The caller does the rest of the hook
+   branch (:2503-2511): intensity, type and SetImageColorspace. */
+MagickBooleanType B200AccelerateGrayscaleImage(Image *image, const PixelIntensityMethod method, ExceptionInfo *exception)
+{
+  enhance_args a;
+  (void) exception;
+  (void) memset(&a, 0, sizeof(a));
+  a.op = 2; a.method = (int) method; a.colorspace = (int) image->colorspace;
+  return run_enhance(image, b200_channels(image), 0u, &a);
+}
+
+/* FunctionImage (statistic.c:1064) on the channels with the Update trait; more than MB200_MAX_FUNCTION_PARAMETERS
+   parameters decline in the library */
+MagickBooleanType B200AccelerateFunctionImage(Image *image, const MagickFunction function, const size_t number_parameters,
+                                              const double *parameters, ExceptionInfo *exception)
+{
+  enhance_args a;
+  unsigned update_mask = 0;
+  const int ch = b200_channels_masked(image, &update_mask);
+  (void) exception;
+  (void) memset(&a, 0, sizeof(a));
+  a.op = 3; a.function = function; a.n = number_parameters; a.params = parameters;
+  return run_enhance(image, ch, update_mask, &a);
+}
+
 static int op_emboss(const float *s, float *d, size_t w, size_t h, int ch, const void *a)
 { const blur_args *b = (const blur_args *) a; return mb200_emboss_image(s, d, w, h, ch, b->radius, b->sigma); }
 
@@ -977,6 +1078,68 @@ MagickBooleanType __wrap_EqualizeImage(Image *image, ExceptionInfo *exception)
 {
   TRY_BOOL(B200AccelerateEqualizeImage(image, exception));
   return __real_EqualizeImage(image, exception);
+}
+
+extern MagickBooleanType __real_ContrastImage(Image *, const MagickBooleanType, ExceptionInfo *);
+extern MagickBooleanType __real_ModulateImage(Image *, const char *, ExceptionInfo *);
+extern MagickBooleanType __real_GrayscaleImage(Image *, const PixelIntensityMethod, ExceptionInfo *);
+extern MagickBooleanType __real_FunctionImage(Image *, const MagickFunction, const size_t, const double *, ExceptionInfo *);
+
+MagickBooleanType __wrap_ContrastImage(Image *image, const MagickBooleanType sharpen, ExceptionInfo *exception)
+{
+  TRY_BOOL(B200AccelerateContrastImage(image, sharpen, exception));
+  return __real_ContrastImage(image, sharpen, exception);
+}
+
+/* ModulateImage's set-up (enhance.c:3677-3710): the re-tag, ParseGeometry and the two artifacts, as the reference does
+   them before its hook */
+MagickBooleanType __wrap_ModulateImage(Image *image, const char *modulate, ExceptionInfo *exception)
+{
+  if (b200_on() && modulate != (const char *) NULL) {
+    ColorspaceType colorspace = UndefinedColorspace;
+    double brightness = 100.0, saturation = 100.0, hue = 100.0;
+    GeometryInfo geometry_info;
+    MagickStatusType flags;
+    const char *artifact;
+    if (IssRGBCompatibleColorspace(image->colorspace) == MagickFalse)
+      (void) SetImageColorspace(image, sRGBColorspace, exception);
+    flags = ParseGeometry(modulate, &geometry_info);
+    if ((flags & RhoValue) != 0) brightness = geometry_info.rho;
+    if ((flags & SigmaValue) != 0) saturation = geometry_info.sigma;
+    if ((flags & XiValue) != 0) hue = geometry_info.xi;
+    artifact = GetImageArtifact(image, "modulate:colorspace");
+    if (artifact != (const char *) NULL)
+      colorspace = (ColorspaceType) ParseCommandOption(MagickColorspaceOptions, MagickFalse, artifact);
+    artifact = GetImageArtifact(image, "color:illuminant");
+    if (artifact != (const char *) NULL && ParseCommandOption(MagickIlluminantOptions, MagickFalse, artifact) < 0)
+      colorspace = UndefinedColorspace;
+    TRY_BOOL(B200AccelerateModulateImage(image, brightness, hue, saturation, colorspace, exception));
+  }
+  return __real_ModulateImage(image, modulate, exception);
+}
+
+/* GrayscaleImage's hook branch (enhance.c:2503-2511) */
+MagickBooleanType __wrap_GrayscaleImage(Image *image, const PixelIntensityMethod method, ExceptionInfo *exception)
+{
+  if (b200_on()) {
+    if (B200AccelerateGrayscaleImage(image, method, exception) != MagickFalse) {
+      B200_COUNT(b200_hits);
+      image->intensity = method;
+      image->type = GrayscaleType;
+      if ((method == Rec601LuminancePixelIntensityMethod) || (method == Rec709LuminancePixelIntensityMethod))
+        return SetImageColorspace(image, LinearGRAYColorspace, exception);
+      return SetImageColorspace(image, GRAYColorspace, exception);
+    }
+    B200_COUNT(b200_fallbacks);
+  }
+  return __real_GrayscaleImage(image, method, exception);
+}
+
+MagickBooleanType __wrap_FunctionImage(Image *image, const MagickFunction function, const size_t number_parameters,
+                                       const double *parameters, ExceptionInfo *exception)
+{
+  TRY_BOOL(B200AccelerateFunctionImage(image, function, number_parameters, parameters, exception));
+  return __real_FunctionImage(image, function, number_parameters, parameters, exception);
 }
 
 extern Image *__real_ScaleImage(const Image *, const size_t, const size_t, ExceptionInfo *);

@@ -19,6 +19,10 @@ extern Image *__real_UnsharpMaskImage(const Image *, const double, const double,
 extern Image *__real_MorphologyImage(const Image *, const MorphologyMethod, const ssize_t, const KernelInfo *, ExceptionInfo *);
 extern Image *__real_ResizeImage(const Image *, const size_t, const size_t, const FilterType, ExceptionInfo *);
 extern MagickBooleanType __real_TransformImageColorspace(Image *, const ColorspaceType, ExceptionInfo *);
+extern MagickBooleanType __real_ContrastImage(Image *, const MagickBooleanType, ExceptionInfo *);
+extern MagickBooleanType __real_ModulateImage(Image *, const char *, ExceptionInfo *);
+extern MagickBooleanType __real_GrayscaleImage(Image *, const PixelIntensityMethod, ExceptionInfo *);
+extern MagickBooleanType __real_FunctionImage(Image *, const MagickFunction, const size_t, const double *, ExceptionInfo *);
 extern Image *__real_SampleImage(const Image *, const size_t, const size_t, ExceptionInfo *);
 extern Image *__real_ScaleImage(const Image *, const size_t, const size_t, ExceptionInfo *);
 extern Image *__real_ThumbnailImage(const Image *, const size_t, const size_t, ExceptionInfo *);
@@ -228,6 +232,51 @@ int main(void)
     }
     if (g) DestroyImage(g);
     if (c) DestroyImage(c);
+  }
+  /* the in-place enhance operators (enhance.c, statistic.c) */
+  a = CloneImage(rgba, 0, 0, MagickTrue, ex); b = CloneImage(rgba, 0, 0, MagickTrue, ex);
+  if (ContrastImage(a, MagickTrue, ex) == MagickFalse) failures++;
+  B200ShimEnable(0); (void) __real_ContrastImage(b, MagickTrue, ex); B200ShimEnable(1);
+  CHECK("ContrastImage(sharpen) RGBA", 1, a, b);
+  a = CloneImage(rgb, 0, 0, MagickTrue, ex); b = CloneImage(rgb, 0, 0, MagickTrue, ex);
+  if (ContrastImage(a, MagickFalse, ex) == MagickFalse) failures++;
+  B200ShimEnable(0); (void) __real_ContrastImage(b, MagickFalse, ex); B200ShimEnable(1);
+  CHECK("ContrastImage(dull) RGB", 1, a, b);
+  a = CloneImage(rgba, 0, 0, MagickTrue, ex); b = CloneImage(rgba, 0, 0, MagickTrue, ex);
+  if (ModulateImage(a, "90,130,150", ex) == MagickFalse) failures++;
+  B200ShimEnable(0); (void) __real_ModulateImage(b, "90,130,150", ex); B200ShimEnable(1);
+  CHECK("ModulateImage 90,130,150 RGBA", 0, a, b);
+  a = CloneImage(rgb, 0, 0, MagickTrue, ex); b = CloneImage(rgb, 0, 0, MagickTrue, ex);
+  (void) SetImageArtifact(a, "modulate:colorspace", "HWB"); (void) SetImageArtifact(b, "modulate:colorspace", "HWB");
+  if (ModulateImage(a, "110x80,40", ex) == MagickFalse) failures++;
+  B200ShimEnable(0); (void) __real_ModulateImage(b, "110x80,40", ex); B200ShimEnable(1);
+  CHECK("ModulateImage HWB 110x80,40 RGB", 0, a, b);
+  a = CloneImage(rgba, 0, 0, MagickTrue, ex); b = CloneImage(rgba, 0, 0, MagickTrue, ex);
+  (void) SetImageArtifact(a, "modulate:colorspace", "LCHab"); (void) SetImageArtifact(b, "modulate:colorspace", "LCHab");
+  (void) SetImageArtifact(a, "color:illuminant", "D50"); (void) SetImageArtifact(b, "color:illuminant", "D50");
+  if (ModulateImage(a, "105,100,140", ex) == MagickFalse) failures++;
+  B200ShimEnable(0); (void) __real_ModulateImage(b, "105,100,140", ex); B200ShimEnable(1);
+  CHECK("ModulateImage LCHab D50 RGBA", 1, a, b);
+  a = CloneImage(rgba, 0, 0, MagickTrue, ex); b = CloneImage(rgba, 0, 0, MagickTrue, ex);
+  if (GrayscaleImage(a, Rec709LuminancePixelIntensityMethod, ex) == MagickFalse || a->colorspace != LinearGRAYColorspace ||
+      GetPixelChannels(a) != 2) failures++;
+  B200ShimEnable(0); (void) __real_GrayscaleImage(b, Rec709LuminancePixelIntensityMethod, ex); B200ShimEnable(1);
+  CHECK("GrayscaleImage Rec709Luminance RGBA", 1, a, b);
+  a = CloneImage(rgb, 0, 0, MagickTrue, ex); b = CloneImage(rgb, 0, 0, MagickTrue, ex);
+  if (GrayscaleImage(a, AveragePixelIntensityMethod, ex) == MagickFalse || a->colorspace != GRAYColorspace ||
+      GetPixelChannels(a) != 1) failures++;
+  B200ShimEnable(0); (void) __real_GrayscaleImage(b, AveragePixelIntensityMethod, ex); B200ShimEnable(1);
+  CHECK("GrayscaleImage Average RGB", 0, a, b);
+  {
+    const double poly[4] = { 0.5, -0.5, 0.75, 0.1 }, sine[2] = { 3.0, 45.0 };
+    a = CloneImage(rgba, 0, 0, MagickTrue, ex); b = CloneImage(rgba, 0, 0, MagickTrue, ex);
+    if (FunctionImage(a, PolynomialFunction, 4, poly, ex) == MagickFalse) failures++;
+    B200ShimEnable(0); (void) __real_FunctionImage(b, PolynomialFunction, 4, poly, ex); B200ShimEnable(1);
+    CHECK("FunctionImage Polynomial RGBA", 0, a, b);
+    a = CloneImage(rgb, 0, 0, MagickTrue, ex); b = CloneImage(rgb, 0, 0, MagickTrue, ex);
+    if (FunctionImage(a, SinusoidFunction, 2, sine, ex) == MagickFalse) failures++;
+    B200ShimEnable(0); (void) __real_FunctionImage(b, SinusoidFunction, 2, sine, ex); B200ShimEnable(1);
+    CHECK("FunctionImage Sinusoid RGB", 1, a, b);
   }
   a = CloneImage(rgba, 0, 0, MagickTrue, ex); b = CloneImage(rgba, 0, 0, MagickTrue, ex);
   if (ClampImage(a, ex) == MagickFalse) failures++;

@@ -453,6 +453,45 @@ MB200_API int mb200_white_threshold_image_dev(float *buf, size_t width, size_t h
 /* ClampImage (:1087): ClampPixel on every channel (HDRI: below 0 -> 0, >= QuantumRange -> QuantumRange). */
 MB200_API int mb200_clamp_image_dev(float *buf, size_t width, size_t height, int channels, void *stream);
 
+/* In-place point operators of MagickCore/enhance.c and statistic.c (the reference's in-place accelerate hooks,
+   accelerate-private.h:50-60), on `buf`.  Gray images (1 or 2 channels) give R, G and B the gray sample; where the three
+   results differ the blue one is written, as in the reference.  Alpha is untouched except by FunctionImage.
+   ContrastImage (enhance.c:1370): HSB brightness pushed along a sine (sharpen != 0) or pulled back (0); <= 1 ULP. */
+MB200_API int mb200_contrast_image_dev(float *buf, size_t width, size_t height, int channels, int sharpen, void *stream);
+/* ModulateImage (enhance.c:3461) with the geometry "B,S,H" already parsed into percentages, `colorspace` the
+   "modulate:colorspace" artifact (HCL, HCLp, HSB, HSI, HSL, HSV, HWB, LCH, LCHab, LCHuv; any other value is HSL) and
+   `illuminant` a value of mb200_illuminant: the "color:illuminant" artifact, used by the LCH spaces (for an unparsable
+   artifact the reference uses D65 and HSL; the caller passes those).  Bit exact in HCL, HCLp, HSB, HSL, HSV and HWB, <= 1 ULP in HSI,
+   LCHab and LCHuv (except the hue noise of achromatic pixels when the chroma is scaled, DESIGN.md §5.8).  The re-tag of an
+   image whose colourspace is not sRGB-compatible (:3681) is the caller's. */
+MB200_API int mb200_modulate_image_dev(float *buf, size_t width, size_t height, int channels, double percent_brightness,
+    double percent_saturation, double percent_hue, int colorspace, int illuminant, void *stream);
+/* MagickCore/pixel.h:110-120 PixelIntensityMethod -- same numeric values */
+typedef enum {
+  MB200_UndefinedPixelIntensityMethod = 0, MB200_AveragePixelIntensityMethod, MB200_BrightnessPixelIntensityMethod,
+  MB200_LightnessPixelIntensityMethod, MB200_MSPixelIntensityMethod, MB200_Rec601LumaPixelIntensityMethod,
+  MB200_Rec601LuminancePixelIntensityMethod, MB200_Rec709LumaPixelIntensityMethod,
+  MB200_Rec709LuminancePixelIntensityMethod, MB200_RMSPixelIntensityMethod
+} mb200_pixel_intensity_method;
+/* GrayscaleImage (enhance.c:2474): the intensity of R, G, B by `method` into channel 0; the other channels are left as
+   they are.  The Luma methods (and Undefined) encode the gamma of a linear-RGB image (`image_colorspace` ==
+   MB200_RGBColorspace), the Luminance methods decode that of an sRGB one.  The caller does the rest of the reference's
+   hook branch (:2503-2511): image->intensity, GrayscaleType, and SetImageColorspace(GRAY, or LinearGRAY for the
+   Luminance methods), which keeps channel 0 (and alpha).  Bit exact without a gamma step, <= 1 ULP with one. */
+MB200_API int mb200_grayscale_image_dev(float *buf, size_t width, size_t height, int channels, int method,
+    int image_colorspace, void *stream);
+/* MagickCore/statistic.h:130-137 MagickFunction -- same numeric values */
+typedef enum {
+  MB200_UndefinedFunction = 0, MB200_ArcsinFunction, MB200_ArctanFunction, MB200_PolynomialFunction,
+  MB200_SinusoidFunction
+} mb200_function;
+#define MB200_MAX_FUNCTION_PARAMETERS 32
+/* FunctionImage (statistic.c:1064) on the channels whose bit is set in `update_mask` (the Update trait: alpha is one of
+   them by default; a `-channel` selection clears the others).  At most MB200_MAX_FUNCTION_PARAMETERS parameters (more:
+   MB200_EUNSUPPORTED, `buf` untouched).  Polynomial and Undefined bit exact, Sinusoid / Arcsin / Arctan <= 1 ULP. */
+MB200_API int mb200_function_image_dev(float *buf, size_t width, size_t height, int channels, int function,
+    size_t number_parameters, const double *parameters, unsigned update_mask, void *stream);
+
 /* Copy-trait channels.  With a `-channel` selection the reference hands the unselected channels through from the
    operator's source (MagickCore/morphology.c:2733-2737, effect.c:4346-4350); ResizeImage takes the nearest source sample
    of each pass (resize.c:3697-3707).  The operators above compute every channel; these point passes put the Copy channels
@@ -528,6 +567,13 @@ MB200_API int mb200_black_threshold_image(float *buf, size_t width, size_t heigh
 MB200_API int mb200_white_threshold_image(float *buf, size_t width, size_t height, int channels,
     int colorspace, const char *thresholds);
 MB200_API int mb200_clamp_image(float *buf, size_t width, size_t height, int channels);
+MB200_API int mb200_contrast_image(float *buf, size_t width, size_t height, int channels, int sharpen);
+MB200_API int mb200_modulate_image(float *buf, size_t width, size_t height, int channels, double percent_brightness,
+    double percent_saturation, double percent_hue, int colorspace, int illuminant);
+MB200_API int mb200_grayscale_image(float *buf, size_t width, size_t height, int channels, int method,
+    int image_colorspace);
+MB200_API int mb200_function_image(float *buf, size_t width, size_t height, int channels, int function,
+    size_t number_parameters, const double *parameters, unsigned update_mask);
 
 #if defined(__cplusplus)
 }

@@ -1,5 +1,5 @@
 """Developer micro-benchmark: device-resident timings of the hot-path operators (CUDA events).
-usage: python tools/devbench.py [blur|resize|lab|dilate|erode|gauss|conv2d|stencils|hooks|all] [size]"""
+usage: python tools/devbench.py [blur|resize|lab|dilate|erode|gauss|conv2d|stencils|hooks|enhance|all] [size]"""
 import sys
 from pathlib import Path
 sys.path.insert(0, str(Path(__file__).resolve().parent.parent))
@@ -118,4 +118,26 @@ if which in ("hooks", "all"):
     print(f"{'LocalContrastImage 10x12.5 ' + str(size) + '^2 RGBA':34s} {ms:9.3f} ms  {fmas / 1e9:.1f} G DFMA  "
           f"{fmas / (ms * 1e-3) / 1e12:.2f} T DFMA/s  {fmas / (ms * 1e-3) / rate.value * 100:5.1f}% of the probed "
           f"{rate.value / 1e12:.2f} T DFMA/s", flush=True)
+    del x
+if which in ("enhance", "all"):
+    # the in-place enhance operators at size^2 RGBA: an in-place pass reads and writes 16 B per pixel (32 B); Grayscale
+    # reads 16 B and writes the 4 B gray sample (20 B).  Share of the 3.35 TB/s H100 SXM data-sheet HBM bandwidth.
+    DATASHEET = 3350.0
+    x = im.Image(torch.rand(size, size, 4, device="cuda") * 65535)
+    for name, fn, bpp in [
+            ("ContrastImage(sharpen)", lambda: im.ContrastImage(x, True), 32),
+            ("ModulateImage 90,120,130 HSL", lambda: im.ModulateImage(x, "90,120,130"), 32),
+            ("ModulateImage 90,120,130 HSB", lambda: im.ModulateImage(x, "90,120,130", {"modulate:colorspace": "HSB"}), 32),
+            ("ModulateImage 90,120,130 LCHab", lambda: im.ModulateImage(x, "90,120,130", {"modulate:colorspace": "LCHab"}), 32),
+            ("GrayscaleImage Rec709Luma", lambda: im.api._in_place(x, "mb200_grayscale_image_dev", "mb200_grayscale_image",
+                                                                   im.Rec709LumaPixelIntensityMethod, im.sRGBColorspace), 20),
+            ("GrayscaleImage Rec709Luminance", lambda: im.api._in_place(x, "mb200_grayscale_image_dev", "mb200_grayscale_image",
+                                                                        im.Rec709LuminancePixelIntensityMethod, im.sRGBColorspace), 20),
+            ("FunctionImage Polynomial 4", lambda: im.FunctionImage(x, im.PolynomialFunction, [0.5, -0.5, 0.75, 0.1]), 32),
+            ("FunctionImage Sinusoid", lambda: im.FunctionImage(x, im.SinusoidFunction, [3.0, 45.0]), 32)]:
+        x.pixels.copy_(torch.rand(size, size, 4, device="cuda") * 65535)
+        ms = timeit(fn, iters=5)
+        gbs = size * size * bpp / ms / 1e6
+        print(f"{name + ' ' + str(size) + '^2 RGBA':44s} {ms:8.3f} ms  {bpp} B/px  {gbs:7.1f} GB/s  "
+              f"{gbs / DATASHEET * 100:5.1f}% of {DATASHEET:.0f} GB/s", flush=True)
     del x
