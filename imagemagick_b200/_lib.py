@@ -101,6 +101,9 @@ PROTOTYPES = {
     "mb200_resize_image": (_i, [_vp, _sz, _sz, _i, _vp, _sz, _sz, _i]),
     "mb200_transform_colorspace": (_i, [_vp, _sz, _sz, _i, _i, _i]),
     "mb200_transform_colorspace_ex": (_i, [_vp, _sz, _sz, _i, _i, _i, _vp]),
+    "mb200_colorspace_channels": (_i, [_i, _i]),
+    "mb200_transform_colorspace_layout_dev": (_i, [_vp, _i, _vp, _i, _sz, _sz, _i, _i, _vp, _vp]),
+    "mb200_transform_colorspace_layout": (_i, [_vp, _i, _vp, _i, _sz, _sz, _i, _i, _vp]),
     "mb200_log_colorspace_table": (_i, [_i, _vp, _vp]),
     "mb200_ycc_table": (_i, [_vp]),
     "mb200_sharpen_kernel": (KernelPtr, [_d, _d]),

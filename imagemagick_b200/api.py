@@ -65,6 +65,9 @@ LogColorspace, YCCColorspace = 15, 28
 LMSColorspace, LuvColorspace, xyYColorspace, DisplayP3Colorspace, Adobe98Colorspace, ProPhotoColorspace, CAT02LMSColorspace = 16, 17, 25, 35, 36, 37, 40
 HCLColorspace, HCLpColorspace, HSBColorspace, HSIColorspace, HSLColorspace, HSVColorspace, HWBColorspace = 4, 5, 6, 7, 8, 9, 10
 GRAYColorspace, LinearGRAYColorspace = 3, 33
+CMYKColorspace = 2
+# the colourspaces whose pixel cache has a channel layout of its own: gray (+ alpha), C M Y K (+ alpha)
+_LAYOUT_SPACES = {GRAYColorspace, LinearGRAYColorspace, CMYKColorspace}
 
 # MagickCore/pixel.h:110-120
 (UndefinedPixelIntensityMethod, AveragePixelIntensityMethod, BrightnessPixelIntensityMethod, LightnessPixelIntensityMethod,
@@ -98,8 +101,8 @@ class Image:
             pixels = np.ascontiguousarray(pixels, dtype=np.float32)
             if pixels.ndim != 3:
                 raise ValueError("pixels must have shape (rows, columns, channels)")
-        if not 1 <= pixels.shape[2] <= 4:
-            raise ValueError("1..4 channels (Gray, Gray+Alpha, RGB, RGBA)")
+        if not 1 <= pixels.shape[2] <= (5 if colorspace == CMYKColorspace else 4):
+            raise ValueError("1..4 channels (Gray, Gray+Alpha, RGB, RGBA), or 5 for CMYK with alpha")
         self.pixels = pixels
         self.colorspace = colorspace
 
@@ -442,6 +445,9 @@ def TransformImageColorspace(image: Image, colorspace: int, settings=None) -> bo
         return True
     opts = colorspace_options_from_settings(settings)
     ref = C.byref(opts) if opts is not None else None
+    if image.colorspace in _LAYOUT_SPACES or colorspace in _LAYOUT_SPACES:
+        _transform_colorspace_layout(image, colorspace, ref)
+        return True
     if image.on_device:
         _activate(image)
         check(lib.mb200_transform_colorspace_ex_dev(image._ptr(), image.columns, image.rows, image.channels,
@@ -451,6 +457,28 @@ def TransformImageColorspace(image: Image, colorspace: int, settings=None) -> bo
                                                 image.colorspace, colorspace, ref))
     image.colorspace = colorspace
     return True
+
+
+def _transform_colorspace_layout(image: Image, colorspace: int, options_ref) -> None:
+    """GRAY, LinearGRAY or CMYK on either side: the pixel cache is replaced by one in the target's channel layout (gray
+    [+ alpha], C M Y K [+ alpha], or three channels [+ alpha]), on the device or on the host like the source."""
+    lib = _lib.load()
+    alpha = image.channels - lib.mb200_colorspace_channels(image.colorspace, 0)
+    out_ch = lib.mb200_colorspace_channels(colorspace, 1 if alpha == 1 else 0)
+    shape = (image.rows, image.columns, out_ch)
+    if image.on_device:
+        import torch
+        out = torch.empty(shape, dtype=torch.float32, device=image.pixels.device)
+        _activate(image)
+        check(lib.mb200_transform_colorspace_layout_dev(image._ptr(), image.channels, out.data_ptr(), out_ch, image.columns,
+                                                        image.rows, image.colorspace, colorspace, options_ref,
+                                                        _stream(image)))
+    else:
+        out = np.empty(shape, dtype=np.float32)
+        check(lib.mb200_transform_colorspace_layout(image._ptr(), image.channels, out.ctypes.data, out_ch, image.columns,
+                                                    image.rows, image.colorspace, colorspace, options_ref))
+    image.pixels = out
+    image.colorspace = colorspace
 
 
 def _in_place(image: Image, dev_fn: str, host_fn: str, *args) -> bool:

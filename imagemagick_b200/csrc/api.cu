@@ -341,21 +341,29 @@ int morphology_apply(const float *src, float *dst, size_t w, size_t h, int ch, i
 // `op(d_src, d_dst, stream)` on the HBM copies of the host buffers (cache.cu): an attached pixel cache keeps its HBM copy
 // between calls (and, in lazy mode, its result stays there until mb200_cache_sync); anything else is staged through
 // stream-ordered temporaries.  Pageable memory travels through the threaded pinned bounce ring.
+// The form with `och` is for operators whose output has its own channel count (the caller checks both counts).
 template <typename Op>
-int with_staging(const char *name, const float *src, size_t w, size_t h, int ch, float *dst, size_t ow, size_t oh, Op op) {
-  if (!src || !dst || !valid_image(w, h, ch) || ow == 0 || oh == 0) return fail(MB200_EINVAL, "%s: bad arguments", name);
+int with_staging(const char *name, const float *src, size_t w, size_t h, int ch, float *dst, size_t ow, size_t oh, int och,
+                 Op op) {
+  if (!src || !dst || w == 0 || h == 0 || ch < 1 || och < 1 || ow == 0 || oh == 0)
+    return fail(MB200_EINVAL, "%s: bad arguments", name);
   cudaStream_t s;
   int rc = prepare(nullptr, &s);
   if (rc) return rc;
   StageRef in, out;
   rc = stage_input(src, image_bytes(w, h, ch), s, &in);
-  if (!rc) rc = stage_output(dst, image_bytes(ow, oh, ch), s, &out);
+  if (!rc) rc = stage_output(dst, image_bytes(ow, oh, och), s, &out);
   if (!rc) rc = op(static_cast<const float *>(in.dev), static_cast<float *>(out.dev), s);
   if (rc) cudaStreamSynchronize(s);
   else rc = finish_output(&out, s);
   release_stage(&in, s);
   release_stage(&out, s);
   return rc;
+}
+template <typename Op>
+int with_staging(const char *name, const float *src, size_t w, size_t h, int ch, float *dst, size_t ow, size_t oh, Op op) {
+  if (!src || !dst || !valid_image(w, h, ch) || ow == 0 || oh == 0) return fail(MB200_EINVAL, "%s: bad arguments", name);
+  return with_staging(name, src, w, h, ch, dst, ow, oh, ch, op);
 }
 
 // In-place operators on a host buffer.
@@ -562,6 +570,22 @@ int mb200_transform_colorspace_dev(float *buf, size_t width, size_t height, int 
   return mb200_transform_colorspace_ex_dev(buf, width, height, channels, from, to, nullptr, stream);
 }
 
+int mb200_colorspace_channels(int colorspace, int has_alpha) {
+  const int base = colorspace == MB200_CMYKColorspace ? 4
+                 : (colorspace == MB200_GRAYColorspace || colorspace == MB200_LinearGRAYColorspace) ? 1 : 3;
+  return base + (has_alpha != 0 ? 1 : 0);
+}
+
+int mb200_transform_colorspace_layout_dev(const float *src, int src_channels, float *dst, int dst_channels, size_t width,
+                                          size_t height, int from, int to, const mb200_colorspace_options *options,
+                                          void *stream) {
+  int rc = colorspace_layout_check(src, src_channels, dst, dst_channels, width, height, from, to, options);
+  cudaStream_t s;
+  if (!rc) rc = prepare(stream, &s);
+  if (rc) return rc;
+  return launch_colorspace_layout(src, src_channels, dst, dst_channels, width * height, from, to, options, s);
+}
+
 // ------------------------------------------------------------ host buffers
 
 int mb200_blur_image(const float *src, float *dst, size_t w, size_t h, int ch, double radius, double sigma) {
@@ -617,6 +641,17 @@ int mb200_transform_colorspace_ex(float *buf, size_t w, size_t h, int ch, int fr
 
 int mb200_transform_colorspace(float *buf, size_t w, size_t h, int ch, int from, int to) {
   return mb200_transform_colorspace_ex(buf, w, h, ch, from, to, nullptr);
+}
+
+// The checks run before the buffers are staged, so a refused call moves no data.
+int mb200_transform_colorspace_layout(const float *src, int src_channels, float *dst, int dst_channels, size_t w, size_t h,
+                                      int from, int to, const mb200_colorspace_options *options) {
+  const int rc = colorspace_layout_check(src, src_channels, dst, dst_channels, w, h, from, to, options);
+  if (rc) return rc;
+  return with_staging("colorspace layout", src, w, h, src_channels, dst, w, h, dst_channels,
+                      [&](const float *s, float *d, cudaStream_t st) {
+                        return launch_colorspace_layout(s, src_channels, d, dst_channels, w * h, from, to, options, st);
+                      });
 }
 
 }  // extern "C"

@@ -723,6 +723,13 @@ int launch_ycc_leg(float *buf, size_t npixels, int channels, bool forward, cudaS
 
 }  // namespace
 
+bool colorspace_served(int cs) {
+  MatrixLeg leg{};
+  return cs == MB200_sRGBColorspace || cs == MB200_RGBColorspace || cs == MB200_XYZColorspace || cs == MB200_LabColorspace ||
+         cs == MB200_LogColorspace || cs == MB200_YCCColorspace || is_hexcone_colorspace(cs) || is_xyz_family(cs) ||
+         matrix_leg(cs, true, leg);
+}
+
 int launch_colorspace(float *buf, size_t npixels, int channels, int from, int to, const mb200_colorspace_options *options,
                       void *stream) {
   if (channels != 3 && channels != 4) return fail(MB200_EUNSUPPORTED, "colorspace: %d channels", channels);

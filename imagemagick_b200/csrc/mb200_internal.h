@@ -170,6 +170,15 @@ int launch_resize_fused(const float *src, size_t width, size_t height, float *ds
 // colorspace.cu
 int launch_colorspace(float *buf, size_t npixels, int channels, int from, int to, const mb200_colorspace_options *options,
                       void *stream);
+// whether launch_colorspace has a leg between `colorspace` and sRGB (sRGB itself included)
+bool colorspace_served(int colorspace);
+
+// layout.cu: TransformImageColorspace to / from GRAY, LinearGRAY and CMYK, out of place (src is never written); the
+// channel counts follow mb200_colorspace_channels.  Every decline is reported before anything is launched.
+int colorspace_layout_check(const void *src, int src_channels, const void *dst, int dst_channels, size_t width,
+                            size_t height, int from, int to, const mb200_colorspace_options *options);
+int launch_colorspace_layout(const float *src, int src_channels, float *dst, int dst_channels, size_t npixels, int from,
+                             int to, const mb200_colorspace_options *options, void *stream);
 
 // hexcone.cu: HCL, HCLp, HSB, HSI, HSL, HSV, HWB (one leg: sRGB -> space or space -> sRGB), in place
 bool is_hexcone_colorspace(int cs);

@@ -86,6 +86,33 @@ static int b200_channels_masked(const Image *image, unsigned *update_mask)
 
 static int b200_channels(const Image *image) { return b200_channels_masked(image, (unsigned *) NULL); }
 
+/* CMYK images (TransformImageColorspace only): cyan, magenta, yellow, black at offsets 0-3 and alpha at 4, every channel
+   with its default traits (pixel.c:6145-6170); 4 or 5 channels. */
+static int b200_cmyk_channels(const Image *image)
+{
+  const size_t n = GetPixelChannels(image);
+  ssize_t i;
+  if (image->colorspace != CMYKColorspace || image->storage_class != DirectClass) return 0;
+  if ((image->channels & (ReadMaskChannel | WriteMaskChannel | CompositeMaskChannel)) != 0) return 0;
+  if (image->number_meta_channels != 0) return 0;
+  if ((GetImageVirtualPixelMethod(image) != UndefinedVirtualPixelMethod) &&
+      (GetImageVirtualPixelMethod(image) != EdgeVirtualPixelMethod)) return 0;
+  if (image->progress_monitor != (MagickProgressMonitor) NULL) return 0;
+  if (GetPixelChannelOffset(image, CyanPixelChannel) != 0 || GetPixelChannelOffset(image, MagentaPixelChannel) != 1 ||
+      GetPixelChannelOffset(image, YellowPixelChannel) != 2 || GetPixelChannelOffset(image, BlackPixelChannel) != 3)
+    return 0;
+  if (!(n == 4 && image->alpha_trait == UndefinedPixelTrait) &&
+      !(n == 5 && image->alpha_trait != UndefinedPixelTrait && GetPixelChannelOffset(image, AlphaPixelChannel) == 4))
+    return 0;
+  for (i = 0; i < (ssize_t) n; i++) {
+    const PixelChannel ch = GetPixelChannelChannel(image, i);
+    const PixelTrait want = (ch == AlphaPixelChannel || image->alpha_trait == UndefinedPixelTrait)
+      ? UpdatePixelTrait : (PixelTrait) (UpdatePixelTrait | BlendPixelTrait);
+    if (GetPixelChannelTraits(image, ch) != want) return 0;
+  }
+  return (int) n;
+}
+
 static MagickBooleanType has_artifact(const Image *image, const char *const *names)
 {
   for (; *names != (const char *) NULL; names++)
@@ -481,6 +508,9 @@ static int map_colorspace(ColorspaceType c)
     case HSLColorspace: return MB200_HSLColorspace;
     case HSVColorspace: return MB200_HSVColorspace;
     case HWBColorspace: return MB200_HWBColorspace;
+    case GRAYColorspace: return MB200_GRAYColorspace;
+    case LinearGRAYColorspace: return MB200_LinearGRAYColorspace;
+    case CMYKColorspace: return MB200_CMYKColorspace;
     default: return -1;
   }
 }
@@ -512,6 +542,65 @@ static MagickBooleanType b200_colorspace_options(const Image *image, mb200_color
   return MagickTrue;
 }
 
+/* GRAY, LinearGRAY or CMYK on either side: the pixel cache changes its channel layout.  The library runs from the current
+   cache into a host buffer in the target layout (a failure there is a clean decline: nothing has changed yet); then
+   SetImageColorspace re-lays the cache out, the buffer is copied into it, and `type` is set as the reference leaves it
+   (GrayscaleType for the gray spaces, colorspace.c:898 / :955; ColorSeparation[Alpha]Type for CMYK, :837-838; otherwise
+   what the pixel sync leaves, as after the reference's own pixel loops). */
+static int b200_source_channels(Image *image, int from)
+{
+  const ColorspaceType saved = image->colorspace;
+  int ch;
+  if (from == MB200_CMYKColorspace) return b200_cmyk_channels(image);
+  if (from == MB200_GRAYColorspace || from == MB200_LinearGRAYColorspace) return b200_channels(image);
+  image->colorspace = sRGBColorspace;          /* the channel layout test is colourspace-agnostic for 3/4-channel images */
+  ch = b200_channels(image);
+  image->colorspace = saved;
+  return ch == 3 || ch == 4 ? ch : 0;
+}
+
+static MagickBooleanType b200_transform_colorspace_layout(Image *image, const ColorspaceType colorspace, int from, int to,
+                                                          const mb200_colorspace_options *copt, ExceptionInfo *exception)
+{
+  const int ch = b200_source_channels(image, from);
+  const size_t n = image->columns * image->rows;
+  int out_ch, rc = MB200_EINVAL;
+  float *buf;
+  const float *p;
+  Quantum *q;
+  MagickBooleanType ok = MagickFalse;
+  if (ch == 0) return MagickFalse;
+  out_ch = mb200_colorspace_channels(to, ch - mb200_colorspace_channels(from, 0));
+  buf = (float *) AcquireQuantumMemory(n, (size_t) out_ch * sizeof(float));
+  if (buf == (float *) NULL) return MagickFalse;
+  {
+    B200_ATTEMPT_BEGIN;
+    p = b200_cache_pixels(image, ch, attempt);
+    if (p != (const float *) NULL)
+      rc = mb200_transform_colorspace_layout(p, ch, buf, out_ch, image->columns, image->rows, from, to,
+                                             copt->set != 0 ? copt : (const mb200_colorspace_options *) NULL);
+    B200_ATTEMPT_END;
+  }
+  if (rc == MB200_OK) {
+    (void) DeleteImageProfile(image, "icc");                 /* colorspace.c:1763-1764 */
+    (void) DeleteImageProfile(image, "icm");
+    if (SetImageColorspace(image, colorspace, exception) != MagickFalse && (int) GetPixelChannels(image) == out_ch) {
+      q = GetAuthenticPixels(image, 0, 0, image->columns, image->rows, exception);
+      if (q != (Quantum *) NULL) {
+        (void) memcpy(q, buf, n * (size_t) out_ch * sizeof(float));
+        ok = SyncAuthenticPixels(image, exception);
+      }
+    }
+    /* the pixel sync resets `type` (as the reference's own loops do); the reference then sets these two */
+    if (colorspace == CMYKColorspace)
+      image->type = image->alpha_trait == UndefinedPixelTrait ? ColorSeparationType : ColorSeparationAlphaType;
+    else if (colorspace == GRAYColorspace || colorspace == LinearGRAYColorspace)
+      image->type = GrayscaleType;
+  }
+  buf = (float *) RelinquishMagickMemory(buf);
+  return ok;
+}
+
 MagickBooleanType B200AccelerateTransformImageColorspace(Image *image, const ColorspaceType colorspace,
                                                          ExceptionInfo *exception)
 {
@@ -522,6 +611,9 @@ MagickBooleanType B200AccelerateTransformImageColorspace(Image *image, const Col
   int ch;
   if (from < 0 || to < 0 || from == to || mb200_device_count() <= 0) return MagickFalse;
   if (b200_colorspace_options(image, &copt, exception) == MagickFalse) return MagickFalse;
+  if (from == MB200_GRAYColorspace || from == MB200_LinearGRAYColorspace || from == MB200_CMYKColorspace ||
+      to == MB200_GRAYColorspace || to == MB200_LinearGRAYColorspace || to == MB200_CMYKColorspace)
+    return b200_transform_colorspace_layout(image, colorspace, from, to, &copt, exception);
   /* the channel layout test is colourspace-agnostic for 3/4-channel images */
   image->colorspace = sRGBColorspace;
   ch = b200_channels(image);

@@ -97,6 +97,36 @@ static Image *noise_image(size_t w, size_t h, MagickBooleanType alpha, Exception
   printf("%-34s max ULP %ld (bar %d)%s\n", name, d_, bar, d_ <= bar ? "" : "  FAIL"); if (d_ > bar) failures++; \
   if (g_) DestroyImage(g_); if (c_) DestroyImage(c_); } while (0)
 
+/* TransformImageColorspace(src -> to) through the shim and through __real_TransformImageColorspace, on clones of `src`:
+   the pixels (within `bar` ULP), the channel count, the colourspace and the image type must agree.  1 on failure. */
+static int layout_case(const char *name, int bar, const Image *src, ColorspaceType to, ExceptionInfo *ex)
+{
+  Image *a = CloneImage(src, 0, 0, MagickTrue, ex), *b = CloneImage(src, 0, 0, MagickTrue, ex);
+  MagickBooleanType ra, rb;
+  long d;
+  ra = TransformImageColorspace(a, to, ex);
+  B200ShimEnable(0); rb = __real_TransformImageColorspace(b, to, ex); B200ShimEnable(1);
+  if (ra == MagickFalse || rb == MagickFalse || a->colorspace != to || b->colorspace != to ||
+      GetPixelChannels(a) != GetPixelChannels(b) || a->type != b->type) {
+    printf("%-34s channels %d/%d colorspace %d/%d type %d/%d  FAIL\n", name, (int) GetPixelChannels(a),
+           (int) GetPixelChannels(b), (int) a->colorspace, (int) b->colorspace, (int) a->type, (int) b->type);
+    d = 1L << 40;
+  } else {
+    d = compare(a, b, ex);
+    printf("%-34s max ULP %ld (bar %d)%s\n", name, d, bar, d <= bar ? "" : "  FAIL");
+  }
+  a = DestroyImage(a); b = DestroyImage(b);
+  return d > bar;
+}
+
+/* a clone of `src` converted by the stock CPU path */
+static Image *converted(const Image *src, ColorspaceType to, ExceptionInfo *ex)
+{
+  Image *im = CloneImage(src, 0, 0, MagickTrue, ex);
+  B200ShimEnable(0); (void) __real_TransformImageColorspace(im, to, ex); B200ShimEnable(1);
+  return im;
+}
+
 int main(void)
 {
   ExceptionInfo *ex;
@@ -192,6 +222,19 @@ int main(void)
   if (TransformImageColorspace(a, sRGBColorspace, ex) == MagickFalse || a->colorspace != sRGBColorspace) failures++;
   B200ShimEnable(0); (void) __real_TransformImageColorspace(b, sRGBColorspace, ex); B200ShimEnable(1);
   CHECK("TransformImageColorspace YCC->sRGB", 0, a, b);
+  {
+    /* the colourspaces that change the channel layout; Lab -> GRAY adds the <= 1 ULP of the Lab leg in R, G and B to a
+       weighted sum that can be several times smaller than one of them */
+    Image *gray = converted(rgb, GRAYColorspace, ex), *cmyka = converted(rgba, CMYKColorspace, ex),
+          *lab = converted(rgba, LabColorspace, ex);
+    failures += layout_case("TransformImageColorspace sRGB->GRAY", 0, rgba, GRAYColorspace, ex);
+    failures += layout_case("TransformImageColorspace sRGB->LinearGRAY", 1, rgb, LinearGRAYColorspace, ex);
+    failures += layout_case("TransformImageColorspace sRGB->CMYK", 0, rgba, CMYKColorspace, ex);
+    failures += layout_case("TransformImageColorspace CMYK->sRGB", 0, cmyka, sRGBColorspace, ex);
+    failures += layout_case("TransformImageColorspace GRAY->sRGB", 0, gray, sRGBColorspace, ex);
+    failures += layout_case("TransformImageColorspace Lab->GRAY", 4, lab, GRAYColorspace, ex);
+    gray = DestroyImage(gray); cmyka = DestroyImage(cmyka); lab = DestroyImage(lab);
+  }
   CHECK("ResizeImage Jinc 50% RGBA", 1, ResizeImage(rgba, rgba->columns / 2, rgba->rows / 2, JincFilter, ex),
         CPU(__real_ResizeImage(rgba, rgba->columns / 2, rgba->rows / 2, JincFilter, ex)));
   (void) SetImageArtifact(rgba, "filter:blur", "0.85"); (void) SetImageArtifact(rgba, "filter:lobes", "2");

@@ -1,5 +1,5 @@
 """Developer micro-benchmark: device-resident timings of the hot-path operators (CUDA events).
-usage: python tools/devbench.py [blur|resize|lab|dilate|erode|gauss|conv2d|stencils|hooks|enhance|all] [size]"""
+usage: python tools/devbench.py [blur|resize|lab|dilate|erode|gauss|conv2d|stencils|hooks|enhance|layout|all] [size]"""
 import sys
 from pathlib import Path
 sys.path.insert(0, str(Path(__file__).resolve().parent.parent))
@@ -141,3 +141,27 @@ if which in ("enhance", "all"):
         print(f"{name + ' ' + str(size) + '^2 RGBA':44s} {ms:8.3f} ms  {bpp} B/px  {gbs:7.1f} GB/s  "
               f"{gbs / DATASHEET * 100:5.1f}% of {DATASHEET:.0f} GB/s", flush=True)
     del x
+if which in ("layout", "all"):
+    # TransformImageColorspace legs that change the channel layout, out of place on device buffers (the entry point
+    # itself, without the Python layer's allocation).  Bytes per pixel: what the leg must read plus write; share of the
+    # 3.35 TB/s H100 SXM data-sheet HBM bandwidth.
+    from imagemagick_b200 import _lib
+    DATASHEET = 3350.0
+    lib = _lib.load()
+    GRAY, LGRAY, CMYK, SRGB, LAB = im.GRAYColorspace, im.LinearGRAYColorspace, im.CMYKColorspace, im.sRGBColorspace, im.LabColorspace
+    import ctypes as C
+    stream = C.c_void_p(torch.cuda.current_stream().cuda_stream or 1)
+    bufs = {ch: torch.rand(size, size, ch, device="cuda") * 65535 for ch in (1, 2, 3, 4, 5)}
+    for name, frm, to, ich, och, bpp in [
+            ("RGBA -> GA", SRGB, GRAY, 4, 2, 24), ("RGBA -> LinearGA", SRGB, LGRAY, 4, 2, 24),
+            ("GA -> RGBA", GRAY, SRGB, 2, 4, 24), ("LinearGA -> RGBA", LGRAY, SRGB, 2, 4, 24),
+            ("RGBA -> CMYKA", SRGB, CMYK, 4, 5, 36), ("CMYKA -> RGBA", CMYK, SRGB, 5, 4, 36),
+            ("RGB -> GRAY", SRGB, GRAY, 3, 1, 16), ("RGB -> CMYK", SRGB, CMYK, 3, 4, 28),
+            ("Lab RGBA -> GA (hop)", LAB, GRAY, 4, 2, 88)]:
+        src, dst = bufs[ich], bufs[och]
+        ms = timeit(lambda: _lib.check(lib.mb200_transform_colorspace_layout_dev(src.data_ptr(), ich, dst.data_ptr(), och, size,
+                                                                                   size, frm, to, None, stream)), iters=9)
+        gbs = size * size * bpp / ms / 1e6
+        print(f"{name + ' ' + str(size) + '^2':44s} {ms:8.3f} ms  {bpp} B/px  {gbs:7.1f} GB/s  "
+              f"{gbs / DATASHEET * 100:5.1f}% of {DATASHEET:.0f} GB/s", flush=True)
+    del bufs
