@@ -165,6 +165,20 @@ PROTOTYPES = {
     "mb200_modulate_image": (_i, [_vp, _sz, _sz, _i, _d, _d, _d, _i, _i]),
     "mb200_grayscale_image": (_i, [_vp, _sz, _sz, _i, _i, _i]),
     "mb200_function_image": (_i, [_vp, _sz, _sz, _i, _i, _sz, C.POINTER(_d), C.c_uint]),
+    "mb200_contrast_stretch_image_dev": (_i, [_vp, _sz, _sz, _i, _d, _d, _i, C.c_uint, _vp, _vp, _vp]),
+    "mb200_contrast_stretch_image": (_i, [_vp, _sz, _sz, _i, _d, _d, _i, C.c_uint, _vp, _vp]),
+    "mb200_linear_stretch_image_dev": (_i, [_vp, _sz, _sz, _i, _d, _d, C.c_uint, _vp, _vp, _vp]),
+    "mb200_linear_stretch_image": (_i, [_vp, _sz, _sz, _i, _d, _d, C.c_uint, _vp, _vp]),
+    "mb200_level_image_dev": (_i, [_vp, _sz, _sz, _i, _d, _d, _d, C.c_uint, _vp]),
+    "mb200_level_image": (_i, [_vp, _sz, _sz, _i, _d, _d, _d, C.c_uint]),
+    "mb200_levelize_image_dev": (_i, [_vp, _sz, _sz, _i, _d, _d, _d, C.c_uint, _vp]),
+    "mb200_levelize_image": (_i, [_vp, _sz, _sz, _i, _d, _d, _d, C.c_uint]),
+    "mb200_minmax_stretch_image_dev": (_i, [_vp, _sz, _sz, _i, _d, _d, _d, _i, C.c_uint, _vp]),
+    "mb200_minmax_stretch_image": (_i, [_vp, _sz, _sz, _i, _d, _d, _d, _i, C.c_uint]),
+    "mb200_gamma_image_dev": (_i, [_vp, _sz, _sz, _i, _d, C.c_uint, _vp]),
+    "mb200_gamma_image": (_i, [_vp, _sz, _sz, _i, _d, C.c_uint]),
+    "mb200_identify_gray_dev": (_i, [_vp, _sz, _sz, _i, _vp, _vp]),
+    "mb200_identify_gray": (_i, [_vp, _sz, _sz, _i, _vp]),
 }
 
 _lib = None

@@ -17,6 +17,9 @@ include/magick_b200.h:
     BilevelImage, BlackThresholdImage, WhiteThresholdImage, ClampImage  threshold.c:805/927/2518/1087
     ContrastImage, ModulateImage, GrayscaleImage                    enhance.c:1370/3461/2474
     FunctionImage                                                   statistic.c:1064
+    LevelImage, LevelizeImage, GammaImage                           enhance.c:2913/3062/2322
+    AutoLevelImage, MinMaxStretchImage                              enhance.c:187, histogram.c:927
+    ContrastStretchImage, NormalizeImage, LinearStretchImage        enhance.c:1544/4130/3347
 
 An `Image` wraps the pixel cache: an (rows, columns, channels) float32 array of raw
 Quantum values (0..65535), either a NumPy array (host; every call stages through
@@ -25,7 +28,8 @@ kernels run on torch's current stream and the result stays in HBM).
 
 Operators that return `Image *` in the reference return a NEW Image here and never
 modify their input; TransformImageColorspace, the threshold operators, Contrast, Modulate,
-Grayscale and Function work in place and return True, like the reference.  Failures raise MagickB200Error (the reference returns NULL / MagickFalse
+Grayscale, Function and the level operators work in place and return True (the stretch operators: their
+"histogram:*" property value), like the reference.  Failures raise MagickB200Error (the reference returns NULL / MagickFalse
 and fills an ExceptionInfo); MB200_EUNSUPPORTED is the "decline" signal on which the
 MagickCore shim falls back to the stock CPU path.  Nothing here computes pixels on
 the CPU.
@@ -583,6 +587,132 @@ def FunctionImage(image: Image, function: int, parameters, channels: Optional[in
     arr = (C.c_double * max(1, len(params)))(*params)
     mask = (1 << image.channels) - 1 if channels is None else int(channels)
     return _in_place(image, "mb200_function_image_dev", "mb200_function_image", int(function), len(params), arr, mask)
+
+
+# ---- level and stretch operators (enhance.c) ------------------------------------------------------------------------
+# `channels` is a `-channel` selection (bit c = channel c has the Update trait); a selection that is given means the
+# image's channel mask is not AllChannels, which switches the histogram operators to per-channel histograms and
+# MinMaxStretch to its per-channel loop even when every channel is selected.
+# colorspace-private.h IssRGBCompatibleColorspace (scRGB 22, Transparent 24)
+_SRGB_COMPATIBLE = (sRGBColorspace, RGBColorspace, DisplayP3Colorspace, Adobe98Colorspace, ProPhotoColorspace, 22, 24,
+                    GRAYColorspace, LinearGRAYColorspace)
+_LINEAR_INTENSITY = (RGBColorspace, LinearGRAYColorspace)     # GetPixelIntensity's Rec709Luma encodes their gamma
+
+
+def _level_mask(image: Image, channels: Optional[int]):
+    """(update_mask, per_channel) of a `channels` selection."""
+    if channels is None:
+        return (1 << image.channels) - 1, 0
+    return int(channels) & ((1 << image.channels) - 1), 1
+
+
+def _check_intensity(image: Image, what: str) -> None:
+    if image.channels > 1 and image.colorspace in _LINEAR_INTENSITY:
+        raise MagickB200Error(_lib.EUNSUPPORTED, f"{what}: the intensity histogram of a linear image is not implemented")
+
+
+def IdentifyImageGray(image: Image) -> int:
+    """The pixel scan of MagickCore/attribute.c:1564 (IsPixelGray / IsPixelMonochrome): 0 not gray, 1 grayscale,
+    2 bilevel.  A colourspace that is not sRGB-compatible is never gray."""
+    if image.colorspace not in _SRGB_COMPATIBLE:
+        return 0
+    kind = C.c_int(0)
+    lib = _lib.load()
+    if image.on_device:
+        _activate(image)
+        check(lib.mb200_identify_gray_dev(image._ptr(), image.columns, image.rows, image.channels, C.byref(kind),
+                                          _stream(image)))
+    else:
+        check(lib.mb200_identify_gray(image._ptr(), image.columns, image.rows, image.channels, C.byref(kind)))
+    return int(kind.value)
+
+
+def _intensity(v, channels: int) -> float:
+    """GetPixelIntensity (pixel.c:2356, Rec709Luma without a gamma step) of a 4-entry array of channel values."""
+    red = float(v[0])
+    if channels == 1:
+        return red
+    green, blue = (float(v[1]), float(v[2])) if channels >= 3 else (red, red)
+    return 0.212656 * red + 0.715158 * green + 0.072186 * blue
+
+
+def ContrastStretchImage(image: Image, black_point: float, white_point: float, channels: Optional[int] = None) -> str:
+    """MagickCore/enhance.c:1544 -- in place; returns the "histogram:contrast-stretch" property.  A gray-valued image
+    (IdentifyImageType, enhance.c:1589-1591) is first re-laid out to the gray channel (plus alpha) and tagged GRAY, as
+    GrayscaleImage's re-layout does."""
+    update_mask, per_channel = _level_mask(image, channels)
+    if IdentifyImageGray(image):
+        if image.channels >= 3:
+            keep = [0, image.channels - 1] if image.channels == 4 else [0]
+            pixels = image.pixels[:, :, keep]
+            image.pixels = pixels.contiguous() if image.on_device else np.ascontiguousarray(pixels)
+            # the selection follows the channels: gray keeps red's bit, alpha its own
+            update_mask = (update_mask & 1) | (2 if len(keep) == 2 and update_mask & 8 else 0)
+        image.colorspace = GRAYColorspace
+    if not per_channel:
+        _check_intensity(image, "contrast stretch")
+    black, white = (C.c_float * 4)(), (C.c_float * 4)()
+    _in_place(image, "mb200_contrast_stretch_image_dev", "mb200_contrast_stretch_image", float(black_point),
+              float(white_point), per_channel, update_mask, black, white)
+    quantum_scale = 1.0 / 65535.0
+    return "%gx%g%%" % (100.0 * quantum_scale * _intensity(black, image.channels),
+                        100.0 * quantum_scale * _intensity(white, image.channels))
+
+
+def NormalizeImage(image: Image, channels: Optional[int] = None) -> str:
+    """MagickCore/enhance.c:4130 -- ContrastStretchImage(0.02 N, 0.99 N) for N pixels."""
+    n = image.columns * image.rows
+    return ContrastStretchImage(image, 0.02 * n, 0.99 * n, channels)
+
+
+def LinearStretchImage(image: Image, black_point: float, white_point: float, channels: Optional[int] = None) -> str:
+    """MagickCore/enhance.c:3347 -- in place (one intensity histogram, then LevelImage on the selected channels); returns
+    the "histogram:linear-stretch" property."""
+    update_mask, _ = _level_mask(image, channels)
+    _check_intensity(image, "linear stretch")
+    black, white = C.c_double(0.0), C.c_double(0.0)
+    _in_place(image, "mb200_linear_stretch_image_dev", "mb200_linear_stretch_image", float(black_point),
+              float(white_point), update_mask, C.byref(black), C.byref(white))
+    return "%gx%g%%" % (100.0 * black.value / 65535, 100.0 * white.value / 65535)
+
+
+def LevelImage(image: Image, black_point: float, white_point: float, gamma: float,
+               channels: Optional[int] = None) -> bool:
+    """MagickCore/enhance.c:2913 -- in place, with its closing ClampImage."""
+    update_mask, _ = _level_mask(image, channels)
+    return _in_place(image, "mb200_level_image_dev", "mb200_level_image", float(black_point), float(white_point),
+                     float(gamma), update_mask)
+
+
+def LevelizeImage(image: Image, black_point: float, white_point: float, gamma: float,
+                  channels: Optional[int] = None) -> bool:
+    """MagickCore/enhance.c:3062 -- in place, no clamp."""
+    update_mask, _ = _level_mask(image, channels)
+    return _in_place(image, "mb200_levelize_image_dev", "mb200_levelize_image", float(black_point), float(white_point),
+                     float(gamma), update_mask)
+
+
+def MinMaxStretchImage(image: Image, black: float, white: float, gamma: float, channels: Optional[int] = None) -> bool:
+    """MagickCore/histogram.c:927 -- GetImageRange, then LevelImage(min + black, max - white, gamma); with a `channels`
+    selection the selected colour channels one at a time.  A CMYK image with a selection is declined: the reference's
+    per-channel loop levels K too, and the library's loop takes the gray / RGB layout."""
+    update_mask, per_channel = _level_mask(image, channels)
+    if per_channel and image.colorspace == CMYKColorspace:
+        raise MagickB200Error(_lib.EUNSUPPORTED, "minmax stretch: a per-channel CMYK image is not implemented")
+    return _in_place(image, "mb200_minmax_stretch_image_dev", "mb200_minmax_stretch_image", float(black), float(white),
+                     float(gamma), per_channel, update_mask)
+
+
+def AutoLevelImage(image: Image, channels: Optional[int] = None) -> bool:
+    """MagickCore/enhance.c:187 -- MinMaxStretchImage(0, 0, 1)."""
+    return MinMaxStretchImage(image, 0.0, 0.0, 1.0, channels)
+
+
+def GammaImage(image: Image, gamma: float, channels: Optional[int] = None) -> bool:
+    """MagickCore/enhance.c:2322 -- in place through the reference's 65 536-entry table; nothing for gamma 1.  (The
+    reference also multiplies image->gamma; an Image here carries no gamma attribute.)"""
+    update_mask, _ = _level_mask(image, channels)
+    return _in_place(image, "mb200_gamma_image_dev", "mb200_gamma_image", float(gamma), update_mask)
 
 
 def MorphologyPrimitive(image: Image, method: int, kernel: Union[str, KernelInfo], bias: float = 0.0):

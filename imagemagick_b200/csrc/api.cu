@@ -1266,3 +1266,145 @@ int mb200_function_image(float *buf, size_t w, size_t h, int ch, int function, s
 }
 
 }  // extern "C"
+
+// ---- level and stretch operators (level.cu) -----------------------------------------------------------------------
+namespace {
+
+unsigned channel_bits(int channels, unsigned update_mask) { return update_mask & ((1u << channels) - 1u); }
+
+// The histograms count in 32 bits (checked before anything is staged, so a refused call moves no data).
+int check_histogram_pixels(size_t w, size_t h, const char *op) {
+  if (w != 0 && h > (((static_cast<size_t>(1) << 32) - 1) / w))
+    return fail(MB200_EUNSUPPORTED, "%s: images of 2^32 pixels or more are not supported", op);
+  return MB200_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int mb200_contrast_stretch_image_dev(float *buf, size_t width, size_t height, int channels, double black_point,
+                                     double white_point, int per_channel, unsigned update_mask, float *black, float *white,
+                                     void *stream) {
+  cudaStream_t s;
+  int rc = prepare_dev(buf && black && white && valid_image(width, height, channels), "contrast stretch", stream, &s);
+  if (!rc) rc = check_histogram_pixels(width, height, "contrast stretch");
+  if (rc) return rc;
+  return launch_contrast_stretch(buf, width, height, channels, black_point, white_point, per_channel != 0,
+                                 channel_bits(channels, update_mask), black, white, s);
+}
+
+int mb200_linear_stretch_image_dev(float *buf, size_t width, size_t height, int channels, double black_point,
+                                   double white_point, unsigned update_mask, double *black_bin, double *white_bin,
+                                   void *stream) {
+  cudaStream_t s;
+  int rc = prepare_dev(buf && black_bin && white_bin && valid_image(width, height, channels), "linear stretch", stream, &s);
+  if (!rc) rc = check_histogram_pixels(width, height, "linear stretch");
+  if (rc) return rc;
+  return launch_linear_stretch(buf, width, height, channels, black_point, white_point, channel_bits(channels, update_mask),
+                               black_bin, white_bin, s);
+}
+
+int mb200_level_image_dev(float *buf, size_t width, size_t height, int channels, double black_point, double white_point,
+                          double gamma, unsigned update_mask, void *stream) {
+  cudaStream_t s;
+  const int rc = prepare_dev(buf && valid_image(width, height, channels), "level", stream, &s);
+  if (rc) return rc;
+  return launch_level(buf, width * height, channels, black_point, white_point, gamma, channel_bits(channels, update_mask),
+                      false, s);
+}
+
+int mb200_levelize_image_dev(float *buf, size_t width, size_t height, int channels, double black_point, double white_point,
+                             double gamma, unsigned update_mask, void *stream) {
+  cudaStream_t s;
+  const int rc = prepare_dev(buf && valid_image(width, height, channels), "levelize", stream, &s);
+  if (rc) return rc;
+  return launch_level(buf, width * height, channels, black_point, white_point, gamma, channel_bits(channels, update_mask),
+                      true, s);
+}
+
+int mb200_minmax_stretch_image_dev(float *buf, size_t width, size_t height, int channels, double black, double white,
+                                   double gamma, int per_channel, unsigned update_mask, void *stream) {
+  cudaStream_t s;
+  const int rc = prepare_dev(buf && valid_image(width, height, channels), "minmax stretch", stream, &s);
+  if (rc) return rc;
+  return launch_minmax_stretch(buf, width, height, channels, black, white, gamma, per_channel != 0,
+                               channel_bits(channels, update_mask), s);
+}
+
+int mb200_gamma_image_dev(float *buf, size_t width, size_t height, int channels, double gamma, unsigned update_mask,
+                          void *stream) {
+  cudaStream_t s;
+  const int rc = prepare_dev(buf && valid_image(width, height, channels), "gamma", stream, &s);
+  if (rc) return rc;
+  return launch_gamma(buf, width * height, channels, gamma, channel_bits(channels, update_mask), s);
+}
+
+int mb200_identify_gray_dev(const float *buf, size_t width, size_t height, int channels, int *type, void *stream) {
+  cudaStream_t s;
+  const int rc = prepare_dev(buf && type && valid_image(width, height, channels), "identify gray", stream, &s);
+  if (rc) return rc;
+  return launch_identify_gray(buf, width * height, channels, type, s);
+}
+
+int mb200_contrast_stretch_image(float *buf, size_t w, size_t h, int ch, double black_point, double white_point,
+                                 int per_channel, unsigned update_mask, float *black, float *white) {
+  int rc = black && white ? check_histogram_pixels(w, h, "contrast stretch") : fail(MB200_EINVAL, "contrast stretch: bad arguments");
+  if (rc) return rc;
+  return in_place_host("contrast stretch", buf, w, h, ch, [&](float *d, cudaStream_t st) {
+    return mb200_contrast_stretch_image_dev(d, w, h, ch, black_point, white_point, per_channel, update_mask, black, white,
+                                            st);
+  });
+}
+
+int mb200_linear_stretch_image(float *buf, size_t w, size_t h, int ch, double black_point, double white_point,
+                               unsigned update_mask, double *black_bin, double *white_bin) {
+  int rc = black_bin && white_bin ? check_histogram_pixels(w, h, "linear stretch")
+                                  : fail(MB200_EINVAL, "linear stretch: bad arguments");
+  if (rc) return rc;
+  return in_place_host("linear stretch", buf, w, h, ch, [&](float *d, cudaStream_t st) {
+    return mb200_linear_stretch_image_dev(d, w, h, ch, black_point, white_point, update_mask, black_bin, white_bin, st);
+  });
+}
+
+int mb200_level_image(float *buf, size_t w, size_t h, int ch, double black_point, double white_point, double gamma,
+                      unsigned update_mask) {
+  return in_place_host("level", buf, w, h, ch, [&](float *d, cudaStream_t st) {
+    return mb200_level_image_dev(d, w, h, ch, black_point, white_point, gamma, update_mask, st);
+  });
+}
+
+int mb200_levelize_image(float *buf, size_t w, size_t h, int ch, double black_point, double white_point, double gamma,
+                         unsigned update_mask) {
+  return in_place_host("levelize", buf, w, h, ch, [&](float *d, cudaStream_t st) {
+    return mb200_levelize_image_dev(d, w, h, ch, black_point, white_point, gamma, update_mask, st);
+  });
+}
+
+int mb200_minmax_stretch_image(float *buf, size_t w, size_t h, int ch, double black, double white, double gamma,
+                               int per_channel, unsigned update_mask) {
+  return in_place_host("minmax stretch", buf, w, h, ch, [&](float *d, cudaStream_t st) {
+    return mb200_minmax_stretch_image_dev(d, w, h, ch, black, white, gamma, per_channel, update_mask, st);
+  });
+}
+
+int mb200_gamma_image(float *buf, size_t w, size_t h, int ch, double gamma, unsigned update_mask) {
+  return in_place_host("gamma", buf, w, h, ch, [&](float *d, cudaStream_t st) {
+    return mb200_gamma_image_dev(d, w, h, ch, gamma, update_mask, st);
+  });
+}
+
+int mb200_identify_gray(const float *buf, size_t w, size_t h, int ch, int *type) {
+  if (!buf || !type || !valid_image(w, h, ch)) return fail(MB200_EINVAL, "identify gray: bad arguments");
+  cudaStream_t s;
+  int rc = prepare(nullptr, &s);
+  if (rc) return rc;
+  StageRef in;                                                   // read only: nothing is copied back
+  rc = stage_input(buf, image_bytes(w, h, ch), s, &in);
+  if (!rc) rc = mb200_identify_gray_dev(static_cast<const float *>(in.dev), w, h, ch, type, s);
+  if (rc) cudaStreamSynchronize(s);
+  release_stage(&in, s);
+  return rc;
+}
+
+}  // extern "C"

@@ -248,6 +248,19 @@ int launch_grayscale(float *buf, size_t npixels, int channels, int method, int i
 int launch_function(float *buf, size_t npixels, int channels, int function, size_t n, const double *params,
                     unsigned update_mask, void *stream);
 
+// level.cu: the level and stretch operators of enhance.c in place, arguments already checked.  contrast / linear stretch
+// read the histogram back (synchronise the stream); identify_gray reads one flag word back.
+int launch_level(float *buf, size_t npixels, int channels, double black, double white, double gamma, unsigned update_mask,
+                 bool levelize, void *stream);
+int launch_minmax_stretch(float *buf, size_t width, size_t height, int channels, double black, double white, double gamma,
+                          bool per_channel, unsigned update_mask, void *stream);
+int launch_contrast_stretch(float *buf, size_t width, size_t height, int channels, double black_point, double white_point,
+                            bool per_channel, unsigned update_mask, float *black, float *white, void *stream);
+int launch_linear_stretch(float *buf, size_t width, size_t height, int channels, double black_point, double white_point,
+                          unsigned update_mask, double *black_bin, double *white_bin, void *stream);
+int launch_gamma(float *buf, size_t npixels, int channels, double gamma, unsigned update_mask, void *stream);
+int launch_identify_gray(const float *buf, size_t npixels, int channels, int *type, void *stream);
+
 // threshold.c point operators in place; op: 0 bilevel (t[0]), 1 black, 2 white (t = r,g,b,a), 3 clamp
 int launch_threshold(float *buf, size_t npixels, int channels, int op, const double *thresholds, void *stream);
 

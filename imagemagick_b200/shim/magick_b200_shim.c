@@ -9,10 +9,12 @@
           --wrap=SharpenImage,--wrap=EdgeImage,--wrap=SampleImage,--wrap=ThumbnailImage,--wrap=MinifyImage,--wrap=ResampleImage,--wrap=MotionBlurImage,\
           --wrap=EmbossImage,--wrap=EqualizeImage,--wrap=StatisticImage,--wrap=RotationalBlurImage,--wrap=BilateralBlurImage,--wrap=ScaleImage,--wrap=SelectiveBlurImage,--wrap=AdaptiveBlurImage,--wrap=AdaptiveSharpenImage,\
           --wrap=DespeckleImage,--wrap=LocalContrastImage,--wrap=WaveletDenoiseImage,\
-          --wrap=ContrastImage,--wrap=ModulateImage,--wrap=GrayscaleImage,--wrap=FunctionImage
+          --wrap=ContrastImage,--wrap=ModulateImage,--wrap=GrayscaleImage,--wrap=FunctionImage,\
+          --wrap=ContrastStretchImage,--wrap=NormalizeImage,--wrap=LinearStretchImage,--wrap=LevelImage,\
+          --wrap=LevelizeImage,--wrap=MinMaxStretchImage,--wrap=GammaImage
   and every caller of those exported functions (effect.c:765/1709/1170/4256, morphology.c:4129,
   resize.c:3761, colorspace.c:1751, threshold.c:805/927/2518/1087, effect.c:1308/2013, visual-effects.c:3515,
-  enhance.c:1370/3461/2474, statistic.c:1064) reaches __wrap_X below.  Each wrapper follows the accelerate
+  enhance.c:1370/3461/2474/1544/4130/3347/2913/3062/2322, histogram.c:927, statistic.c:1064) reaches __wrap_X below.  Each wrapper follows the accelerate
   hook contract of effect.c:783-787 / resize.c:3818-3826: try the GPU; if the image is not
   eligible or the GPU path declines (returns NULL / MagickFalse without raising), run the stock
   CPU implementation (__real_X).  B200Accelerate*Image() are the same functions with the
@@ -843,6 +845,154 @@ MagickBooleanType B200AccelerateFunctionImage(Image *image, const MagickFunction
   return run_enhance(image, ch, update_mask, &a);
 }
 
+/* ---- level and stretch operators (enhance.c; AccelerateContrastStretchImage is accelerate-private.h:52) ------------------
+   b200_channels_masked gives the Update channels and declines PseudoClass (the colormap step stays on the CPU path), CMYK
+   and the rest.  The histogram operators index the histogram by GetPixelIntensity: equalize_eligible. */
+typedef struct {
+  int op;                       /* 0 level, 1 levelize, 2 minmax stretch, 3 gamma, 4 contrast stretch, 5 linear stretch */
+  double a, b, gamma;
+  float black[4], white[4];     /* contrast stretch: the bins per channel */
+  double black_bin, white_bin;  /* linear stretch */
+} level_args;
+
+static MagickBooleanType run_level(Image *image, level_args *a)
+{
+  MagickBooleanType ok = MagickFalse;
+  unsigned update_mask = 0;
+  const int ch = b200_channels_masked(image, &update_mask);
+  const int per_channel = image->channel_mask != AllChannels ? 1 : 0;
+  Quantum *q;
+  int rc = MB200_EINVAL;
+  if (ch == 0 || mb200_device_count() <= 0) return MagickFalse;
+  {
+    B200_ATTEMPT_BEGIN;
+    q = GetAuthenticPixels(image, 0, 0, image->columns, image->rows, attempt);
+    if (q != (Quantum *) NULL && b200_cache_pixels(image, ch, attempt) == (float *) q) {
+      float *buf = (float *) q;
+      const size_t w = image->columns, h = image->rows;
+      switch (a->op) {
+        case 0: rc = mb200_level_image(buf, w, h, ch, a->a, a->b, a->gamma, update_mask); break;
+        case 1: rc = mb200_levelize_image(buf, w, h, ch, a->a, a->b, a->gamma, update_mask); break;
+        case 2: rc = mb200_minmax_stretch_image(buf, w, h, ch, a->a, a->b, a->gamma, per_channel, update_mask); break;
+        case 3: rc = mb200_gamma_image(buf, w, h, ch, a->gamma, update_mask); break;
+        case 4:
+          rc = mb200_contrast_stretch_image(buf, w, h, ch, a->a, a->b, per_channel, update_mask, a->black, a->white);
+          break;
+        default:
+          rc = mb200_linear_stretch_image(buf, w, h, ch, a->a, a->b, update_mask, &a->black_bin, &a->white_bin);
+          break;
+      }
+    }
+    /* on failure nothing was written back: the CPU path starts from the same pixels */
+    if (rc == MB200_OK && SyncAuthenticPixels(image, attempt) != MagickFalse) ok = MagickTrue;
+    B200_ATTEMPT_END;
+  }
+  return ok;
+}
+
+MagickBooleanType B200AccelerateLevelImage(Image *image, const double black_point, const double white_point,
+                                           const double gamma, ExceptionInfo *exception)
+{
+  level_args a;
+  (void) exception;
+  (void) memset(&a, 0, sizeof(a));
+  a.op = 0; a.a = black_point; a.b = white_point; a.gamma = gamma;
+  return run_level(image, &a);
+}
+
+MagickBooleanType B200AccelerateLevelizeImage(Image *image, const double black_point, const double white_point,
+                                              const double gamma, ExceptionInfo *exception)
+{
+  level_args a;
+  (void) exception;
+  (void) memset(&a, 0, sizeof(a));
+  a.op = 1; a.a = black_point; a.b = white_point; a.gamma = gamma;
+  return run_level(image, &a);
+}
+
+/* MinMaxStretchImage (histogram.c:927), AutoLevelImage's body: the per-channel loop runs in the library */
+MagickBooleanType B200AccelerateMinMaxStretchImage(Image *image, const double black, const double white,
+                                                   const double gamma, ExceptionInfo *exception)
+{
+  level_args a;
+  (void) exception;
+  (void) memset(&a, 0, sizeof(a));
+  a.op = 2; a.a = black; a.b = white; a.gamma = gamma;
+  return run_level(image, &a);
+}
+
+/* GammaImage (enhance.c:2322), with its image->gamma update (:2441-2442) */
+MagickBooleanType B200AccelerateGammaImage(Image *image, const double gamma, ExceptionInfo *exception)
+{
+  level_args a;
+  (void) exception;
+  (void) memset(&a, 0, sizeof(a));
+  a.op = 3; a.gamma = gamma;
+  if (run_level(image, &a) == MagickFalse) return MagickFalse;
+  if (gamma != 1.0 && image->gamma != 0.0) image->gamma *= gamma;
+  return MagickTrue;
+}
+
+/* ContrastStretchImage (enhance.c:1544) with the reference's control plane: IdentifyImageType's gray test (:1589-1591; the
+   pixel scan on the device), SetImageColorspace(GRAY), the stretch, then the property with the reference's own
+   GetPixelIntensity and FormatLocaleString (:1810-1814). */
+MagickBooleanType B200AccelerateContrastStretchImage(Image *image, const double black_point, const double white_point,
+                                                     ExceptionInfo *exception)
+{
+  level_args a;
+  Quantum black[MaxPixelChannels], white[MaxPixelChannels];
+  char property[MagickPathExtent];
+  unsigned mask = 0;
+  int ch, i, gray = 0;
+  if (mb200_device_count() <= 0) return MagickFalse;
+  if (image->channel_mask == AllChannels && equalize_eligible(image) == MagickFalse) return MagickFalse;
+  ch = b200_channels_masked(image, &mask);
+  if (ch == 0) return MagickFalse;
+  if (IsImageGray(image) != MagickFalse) gray = 1;                     /* IdentifyImageGray (attribute.c:1583-1584) */
+  else if (IssRGBCompatibleColorspace(image->colorspace) != MagickFalse) {
+    /* the cache itself (its HBM copy when attached): no GetVirtualPixels, which would pull a resident result back */
+    const float *p = b200_cache_pixels(image, ch, exception);
+    int type = 0;
+    if (p == (const float *) NULL || mb200_identify_gray(p, image->columns, image->rows, ch, &type) != MB200_OK)
+      return MagickFalse;
+    gray = type != 0;
+  }
+  if (gray != 0) (void) SetImageColorspace(image, GRAYColorspace, exception);
+  (void) memset(&a, 0, sizeof(a));
+  a.op = 4; a.a = black_point; a.b = white_point;
+  if (run_level(image, &a) == MagickFalse) return MagickFalse;
+  (void) memset(black, 0, sizeof(black));
+  (void) memset(white, 0, sizeof(white));
+  for (i = 0; i < 4; i++) { black[i] = (Quantum) a.black[i]; white[i] = (Quantum) a.white[i]; }
+  (void) FormatLocaleString(property, MagickPathExtent, "%gx%g%%", 100.0 * QuantumScale * GetPixelIntensity(image, black),
+                            100.0 * QuantumScale * GetPixelIntensity(image, white));
+  (void) SetImageProperty(image, "histogram:contrast-stretch", property, exception);
+  return MagickTrue;
+}
+
+/* NormalizeImage (enhance.c:4130): its ContrastStretchImage call stays inside enhance.o, so it is wrapped itself */
+MagickBooleanType B200AccelerateNormalizeImage(Image *image, ExceptionInfo *exception)
+{
+  const double black_point = 0.02 * image->columns * image->rows, white_point = 0.99 * image->columns * image->rows;
+  return B200AccelerateContrastStretchImage(image, black_point, white_point, exception);
+}
+
+/* LinearStretchImage (enhance.c:3347): one intensity histogram, LevelImage, the property (:3421-3424) */
+MagickBooleanType B200AccelerateLinearStretchImage(Image *image, const double black_point, const double white_point,
+                                                   ExceptionInfo *exception)
+{
+  level_args a;
+  char property[MagickPathExtent];
+  if (equalize_eligible(image) == MagickFalse) return MagickFalse;
+  (void) memset(&a, 0, sizeof(a));
+  a.op = 5; a.a = black_point; a.b = white_point;
+  if (run_level(image, &a) == MagickFalse) return MagickFalse;
+  (void) FormatLocaleString(property, MagickPathExtent, "%gx%g%%", 100.0 * (ssize_t) a.black_bin / MaxMap,
+                            100.0 * (ssize_t) a.white_bin / MaxMap);
+  (void) SetImageProperty(image, "histogram:linear-stretch", property, exception);
+  return MagickTrue;
+}
+
 static int op_emboss(const float *s, float *d, size_t w, size_t h, int ch, const void *a)
 { const blur_args *b = (const blur_args *) a; return mb200_emboss_image(s, d, w, h, ch, b->radius, b->sigma); }
 
@@ -1232,6 +1382,61 @@ MagickBooleanType __wrap_FunctionImage(Image *image, const MagickFunction functi
 {
   TRY_BOOL(B200AccelerateFunctionImage(image, function, number_parameters, parameters, exception));
   return __real_FunctionImage(image, function, number_parameters, parameters, exception);
+}
+
+extern MagickBooleanType __real_ContrastStretchImage(Image *, const double, const double, ExceptionInfo *);
+extern MagickBooleanType __real_NormalizeImage(Image *, ExceptionInfo *);
+extern MagickBooleanType __real_LinearStretchImage(Image *, const double, const double, ExceptionInfo *);
+extern MagickBooleanType __real_LevelImage(Image *, const double, const double, const double, ExceptionInfo *);
+extern MagickBooleanType __real_LevelizeImage(Image *, const double, const double, const double, ExceptionInfo *);
+extern MagickBooleanType __real_MinMaxStretchImage(Image *, const double, const double, const double, ExceptionInfo *);
+extern MagickBooleanType __real_GammaImage(Image *, const double, ExceptionInfo *);
+
+MagickBooleanType __wrap_ContrastStretchImage(Image *image, const double black_point, const double white_point,
+                                              ExceptionInfo *exception)
+{
+  TRY_BOOL(B200AccelerateContrastStretchImage(image, black_point, white_point, exception));
+  return __real_ContrastStretchImage(image, black_point, white_point, exception);
+}
+
+MagickBooleanType __wrap_NormalizeImage(Image *image, ExceptionInfo *exception)
+{
+  TRY_BOOL(B200AccelerateNormalizeImage(image, exception));
+  return __real_NormalizeImage(image, exception);
+}
+
+MagickBooleanType __wrap_LinearStretchImage(Image *image, const double black_point, const double white_point,
+                                            ExceptionInfo *exception)
+{
+  TRY_BOOL(B200AccelerateLinearStretchImage(image, black_point, white_point, exception));
+  return __real_LinearStretchImage(image, black_point, white_point, exception);
+}
+
+MagickBooleanType __wrap_LevelImage(Image *image, const double black_point, const double white_point, const double gamma,
+                                    ExceptionInfo *exception)
+{
+  TRY_BOOL(B200AccelerateLevelImage(image, black_point, white_point, gamma, exception));
+  return __real_LevelImage(image, black_point, white_point, gamma, exception);
+}
+
+MagickBooleanType __wrap_LevelizeImage(Image *image, const double black_point, const double white_point, const double gamma,
+                                       ExceptionInfo *exception)
+{
+  TRY_BOOL(B200AccelerateLevelizeImage(image, black_point, white_point, gamma, exception));
+  return __real_LevelizeImage(image, black_point, white_point, gamma, exception);
+}
+
+MagickBooleanType __wrap_MinMaxStretchImage(Image *image, const double black, const double white, const double gamma,
+                                            ExceptionInfo *exception)
+{
+  TRY_BOOL(B200AccelerateMinMaxStretchImage(image, black, white, gamma, exception));
+  return __real_MinMaxStretchImage(image, black, white, gamma, exception);
+}
+
+MagickBooleanType __wrap_GammaImage(Image *image, const double gamma, ExceptionInfo *exception)
+{
+  TRY_BOOL(B200AccelerateGammaImage(image, gamma, exception));
+  return __real_GammaImage(image, gamma, exception);
 }
 
 extern Image *__real_ScaleImage(const Image *, const size_t, const size_t, ExceptionInfo *);

@@ -48,6 +48,12 @@ extern MagickBooleanType __real_BilevelImage(Image *, const double, ExceptionInf
 extern MagickBooleanType __real_BlackThresholdImage(Image *, const char *, ExceptionInfo *);
 extern MagickBooleanType __real_WhiteThresholdImage(Image *, const char *, ExceptionInfo *);
 extern MagickBooleanType __real_ClampImage(Image *, ExceptionInfo *);
+extern MagickBooleanType __real_ContrastStretchImage(Image *, const double, const double, ExceptionInfo *);
+extern MagickBooleanType __real_NormalizeImage(Image *, ExceptionInfo *);
+extern MagickBooleanType __real_LinearStretchImage(Image *, const double, const double, ExceptionInfo *);
+extern MagickBooleanType __real_LevelImage(Image *, const double, const double, const double, ExceptionInfo *);
+extern MagickBooleanType __real_LevelizeImage(Image *, const double, const double, const double, ExceptionInfo *);
+extern MagickBooleanType __real_GammaImage(Image *, const double, ExceptionInfo *);
 extern long B200ShimHits(void), B200ShimFallbacks(void);
 extern void B200ShimEnable(int);
 
@@ -125,6 +131,51 @@ static Image *converted(const Image *src, ColorspaceType to, ExceptionInfo *ex)
   Image *im = CloneImage(src, 0, 0, MagickTrue, ex);
   B200ShimEnable(0); (void) __real_TransformImageColorspace(im, to, ex); B200ShimEnable(1);
   return im;
+}
+
+
+/* The level and stretch operators on clones of `src` (under SetPixelChannelMask(mask) when mask >= 0): through the shim
+   and through the stock CPU path.  The pixels (within `bar` ULP), the channel count, the colourspace, the "histogram:*"
+   properties and image->gamma must agree; with `expect_fallback` the shim must have declined.  1 on failure.
+   op: 0 Level, 1 Levelize, 2 Gamma, 3 AutoLevel (MinMaxStretchImage, wrapped), 4 ContrastStretch, 5 Normalize,
+   6 LinearStretch. */
+static MagickBooleanType level_op(Image *im, int op, double x, double y, double g, int cpu, ExceptionInfo *ex)
+{
+  switch (op) {
+    case 0: return cpu ? __real_LevelImage(im, x, y, g, ex) : LevelImage(im, x, y, g, ex);
+    case 1: return cpu ? __real_LevelizeImage(im, x, y, g, ex) : LevelizeImage(im, x, y, g, ex);
+    case 2: return cpu ? __real_GammaImage(im, g, ex) : GammaImage(im, g, ex);
+    case 3: return AutoLevelImage(im, ex);        /* its MinMaxStretchImage call is wrapped; the CPU side disables the shim */
+    case 4: return cpu ? __real_ContrastStretchImage(im, x, y, ex) : ContrastStretchImage(im, x, y, ex);
+    case 5: return cpu ? __real_NormalizeImage(im, ex) : NormalizeImage(im, ex);
+    default: return cpu ? __real_LinearStretchImage(im, x, y, ex) : LinearStretchImage(im, x, y, ex);
+  }
+}
+
+static int level_case(const char *name, int bar, const Image *src, int op, double x, double y, double g, long mask,
+                      int expect_fallback, ExceptionInfo *ex)
+{
+  static const char *const props[] = { "histogram:contrast-stretch", "histogram:linear-stretch" };
+  Image *a = CloneImage(src, 0, 0, MagickTrue, ex), *b = CloneImage(src, 0, 0, MagickTrue, ex);
+  const long fb = B200ShimFallbacks();
+  MagickBooleanType ra, rb;
+  long d = 0;
+  int k, bad = 0;
+  if (mask >= 0) { (void) SetPixelChannelMask(a, (ChannelType) mask); (void) SetPixelChannelMask(b, (ChannelType) mask); }
+  ra = level_op(a, op, x, y, g, 0, ex);
+  B200ShimEnable(0); rb = level_op(b, op, x, y, g, 1, ex); B200ShimEnable(1);
+  if (ra == MagickFalse || rb == MagickFalse || GetPixelChannels(a) != GetPixelChannels(b) ||
+      a->colorspace != b->colorspace || a->gamma != b->gamma) bad = 1;
+  for (k = 0; k < 2; k++) {
+    const char *pa = GetImageProperty(a, props[k], ex), *pb = GetImageProperty(b, props[k], ex);
+    if ((pa == NULL) != (pb == NULL) || (pa != NULL && strcmp(pa, pb) != 0)) bad = 1;
+  }
+  if (!bad) d = compare(a, b, ex);
+  if (expect_fallback && mb200_device_count() > 0 && B200ShimFallbacks() <= fb) bad = 1;
+  printf("%-34s max ULP %ld (bar %d) channels %d/%d%s\n", name, d, bar, (int) GetPixelChannels(a),
+         (int) GetPixelChannels(b), bad || d > bar ? "  FAIL" : "");
+  a = DestroyImage(a); b = DestroyImage(b);
+  return bad || d > bar;
 }
 
 int main(void)
@@ -320,6 +371,46 @@ int main(void)
     if (FunctionImage(a, SinusoidFunction, 2, sine, ex) == MagickFalse) failures++;
     B200ShimEnable(0); (void) __real_FunctionImage(b, SinusoidFunction, 2, sine, ex); B200ShimEnable(1);
     CHECK("FunctionImage Sinusoid RGB", 1, a, b);
+  }
+  {
+    /* level and stretch operators (enhance.c, histogram.c:927): in place, the reference's control plane around them */
+    const long hits0 = B200ShimHits();
+    Image *gray = CloneImage(rgba, 0, 0, MagickTrue, ex), *t;
+    Quantum *q = GetAuthenticPixels(gray, 0, 0, gray->columns, gray->rows, ex);
+    size_t i;
+    for (i = 0; i < gray->columns * gray->rows; i++) { q[4 * i + 1] = q[4 * i]; q[4 * i + 2] = q[4 * i]; }
+    (void) SyncAuthenticPixels(gray, ex);
+    failures += level_case("LevelImage 1000,60000,1 RGBA", 0, rgba, 0, 1000.0, 60000.0, 1.0, -1, 0, ex);
+    failures += level_case("LevelImage 5000,50000,2.2 RGB", 1, rgb, 0, 5000.0, 50000.0, 2.2, -1, 0, ex);
+    failures += level_case("LevelizeImage 1000,60000,0.45 RGBA", 1, rgba, 1, 1000.0, 60000.0, 0.45, -1, 0, ex);
+    failures += level_case("LevelImage -channel RBA RGBA", 0, rgba, 0, 2000.0, 50000.0, 1.0,
+                           RedChannel | BlueChannel | AlphaChannel, 0, ex);
+    failures += level_case("GammaImage 2.2 RGBA", 0, rgba, 2, 0.0, 0.0, 2.2, -1, 0, ex);
+    failures += level_case("GammaImage 0.45 RGB", 0, rgb, 2, 0.0, 0.0, 0.45, -1, 0, ex);
+    failures += level_case("AutoLevelImage RGBA", 0, rgba, 3, 0.0, 0.0, 1.0, -1, 0, ex);
+    failures += level_case("AutoLevelImage -channel RGBA", 0, rgba, 3, 0.0, 0.0, 1.0,
+                           RedChannel | GreenChannel | BlueChannel | AlphaChannel, 0, ex);
+    failures += level_case("ContrastStretchImage 1%,97% RGBA", 0, rgba, 4, 0.01 * 517 * 389, 0.97 * 517 * 389, 1.0, -1, 0, ex);
+    failures += level_case("ContrastStretchImage -channel RGBA", 0, rgba, 4, 0.05 * 517 * 389, 0.9 * 517 * 389, 1.0,
+                           RedChannel | GreenChannel | BlueChannel | AlphaChannel, 0, ex);
+    failures += level_case("NormalizeImage RGB", 0, rgb, 5, 0.0, 0.0, 1.0, -1, 0, ex);
+    failures += level_case("NormalizeImage gray sRGBA -> GA", 0, gray, 5, 0.0, 0.0, 1.0, -1, 0, ex);
+    failures += level_case("LinearStretchImage 2%,1% RGBA", 0, rgba, 6, 0.02 * 517 * 389, 0.01 * 517 * 389, 1.0, -1, 0, ex);
+    if (mb200_device_count() > 0 && B200ShimHits() - hits0 < 13) { printf("FAIL: level operators did not reach the GPU path\n"); failures++; }
+    /* the fallbacks: PseudoClass, a linear-RGB image's intensity histogram, a non-default intensity method */
+    t = CloneImage(rgb, 0, 0, MagickTrue, ex);
+    (void) SetImageType(t, PaletteType, ex);         /* quantised to a colormap: PseudoClass */
+    failures += level_case("fallback: LevelImage PseudoClass", 0, t, 0, 1000.0, 60000.0, 1.0, -1, 1, ex);
+    t = DestroyImage(t);
+    t = CloneImage(rgb, 0, 0, MagickTrue, ex);
+    t->colorspace = RGBColorspace;
+    failures += level_case("fallback: NormalizeImage linear RGB", 0, t, 5, 0.0, 0.0, 1.0, -1, 1, ex);
+    t = DestroyImage(t);
+    t = CloneImage(rgba, 0, 0, MagickTrue, ex);
+    t->intensity = AveragePixelIntensityMethod;
+    failures += level_case("fallback: LinearStretch Average", 0, t, 6, 0.02 * 517 * 389, 0.01 * 517 * 389, 1.0, -1, 1, ex);
+    t = DestroyImage(t);
+    gray = DestroyImage(gray);
   }
   a = CloneImage(rgba, 0, 0, MagickTrue, ex); b = CloneImage(rgba, 0, 0, MagickTrue, ex);
   if (ClampImage(a, ex) == MagickFalse) failures++;

@@ -509,6 +509,46 @@ typedef enum {
    MB200_EUNSUPPORTED, `buf` untouched).  Polynomial and Undefined bit exact, Sinusoid / Arcsin / Arctan <= 1 ULP. */
 MB200_API int mb200_function_image_dev(float *buf, size_t width, size_t height, int channels, int function,
     size_t number_parameters, const double *parameters, unsigned update_mask, void *stream);
+/* The level and stretch operators of enhance.c, in place.  `update_mask`: bit c = channel c has the Update trait (all
+   channels, alpha included, by default).  `per_channel`: the image's channel mask is not AllChannels (a `-channel`
+   selection, even one that leaves every trait at its default).  Bad arguments give MB200_EINVAL, unsupported cases
+   MB200_EUNSUPPORTED; both leave `buf` untouched.
+   ContrastStretchImage (enhance.c:1544; NormalizeImage is black 0.02 N, white 0.99 N for N pixels): one intensity
+   histogram (Rec709Luma, no gamma step: the caller declines linear images and other intensity methods) for every
+   channel, or one per channel with `per_channel`; black / white bins per channel ([4], unused entries 0) are returned
+   for the "histogram:contrast-stretch" property.  IdentifyImageType's gray re-layout (SetImageColorspace(GRAY) of a
+   gray-valued image) is the caller's, before the call: see mb200_identify_gray_dev.  Bit exact.  Reads the histogram
+   back, so it synchronises `stream`.  Images of 2^32 pixels or more: MB200_EUNSUPPORTED. */
+MB200_API int mb200_contrast_stretch_image_dev(float *buf, size_t width, size_t height, int channels, double black_point,
+    double white_point, int per_channel, unsigned update_mask, float *black, float *white, void *stream);
+/* LinearStretchImage (enhance.c:3347): one intensity histogram, black / white bins by its own search (returned for the
+   "histogram:linear-stretch" property), then LevelImage(black, white, 1) on the Update channels.  Bit exact.
+   Synchronises `stream`; 2^32 pixels or more: MB200_EUNSUPPORTED. */
+MB200_API int mb200_linear_stretch_image_dev(float *buf, size_t width, size_t height, int channels, double black_point,
+    double white_point, unsigned update_mask, double *black_bin, double *white_bin, void *stream);
+/* LevelImage (enhance.c:2913, with its closing ClampImage) and LevelizeImage (:3062, no clamp) on the Update channels.
+   Bit exact at gamma 1, <= 1 ULP otherwise (CUDA pow).  Asynchronous. */
+MB200_API int mb200_level_image_dev(float *buf, size_t width, size_t height, int channels, double black_point,
+    double white_point, double gamma, unsigned update_mask, void *stream);
+MB200_API int mb200_levelize_image_dev(float *buf, size_t width, size_t height, int channels, double black_point,
+    double white_point, double gamma, unsigned update_mask, void *stream);
+/* MinMaxStretchImage (histogram.c:927; AutoLevelImage is black 0, white 0, gamma 1): GetImageRange, each row seeded by
+   its first sample of channel 0, then LevelImage(min + black, max - white, gamma) when the two differ by MagickEpsilon
+   or more.  With `per_channel` the Update colour channels one at a time in channel order (range, then level); alpha is
+   never levelled there, as in the reference.  The per-channel loop takes the gray / RGB layout (colour channels at
+   offsets 0-2, alpha last); a CMYK image's K would be levelled by the reference and is the caller's to decline.  The decision is taken on the device: asynchronous.  Bit exact at gamma 1. */
+MB200_API int mb200_minmax_stretch_image_dev(float *buf, size_t width, size_t height, int channels, double black,
+    double white, double gamma, int per_channel, unsigned update_mask, void *stream);
+/* GammaImage (enhance.c:2322): nothing for gamma 1; otherwise the reference's 65 536-entry table (built on the host with
+   libm; all zeros for gamma 0) on the Update channels.  Bit exact.  The caller multiplies image->gamma.  Nothing is read
+   back, but the table is a pageable upload, which CUDA orders after the work already queued on `stream`: the call
+   returns once that work is done and the table is on the device. */
+MB200_API int mb200_gamma_image_dev(float *buf, size_t width, size_t height, int channels, double gamma,
+    unsigned update_mask, void *stream);
+/* IdentifyImageGray's pixel scan (attribute.c:1564-1626; IsPixelGray / IsPixelMonochrome on channels 0-2, or the gray
+   sample three times for 1-2 channels): *type = 0 not gray, 1 grayscale, 2 bilevel.  Synchronises `stream`. */
+MB200_API int mb200_identify_gray_dev(const float *buf, size_t width, size_t height, int channels, int *type,
+    void *stream);
 
 /* Copy-trait channels.  With a `-channel` selection the reference hands the unselected channels through from the
    operator's source (MagickCore/morphology.c:2733-2737, effect.c:4346-4350); ResizeImage takes the nearest source sample
@@ -594,6 +634,19 @@ MB200_API int mb200_grayscale_image(float *buf, size_t width, size_t height, int
     int image_colorspace);
 MB200_API int mb200_function_image(float *buf, size_t width, size_t height, int channels, int function,
     size_t number_parameters, const double *parameters, unsigned update_mask);
+MB200_API int mb200_contrast_stretch_image(float *buf, size_t width, size_t height, int channels, double black_point,
+    double white_point, int per_channel, unsigned update_mask, float *black, float *white);
+MB200_API int mb200_linear_stretch_image(float *buf, size_t width, size_t height, int channels, double black_point,
+    double white_point, unsigned update_mask, double *black_bin, double *white_bin);
+MB200_API int mb200_level_image(float *buf, size_t width, size_t height, int channels, double black_point,
+    double white_point, double gamma, unsigned update_mask);
+MB200_API int mb200_levelize_image(float *buf, size_t width, size_t height, int channels, double black_point,
+    double white_point, double gamma, unsigned update_mask);
+MB200_API int mb200_minmax_stretch_image(float *buf, size_t width, size_t height, int channels, double black,
+    double white, double gamma, int per_channel, unsigned update_mask);
+MB200_API int mb200_gamma_image(float *buf, size_t width, size_t height, int channels, double gamma,
+    unsigned update_mask);
+MB200_API int mb200_identify_gray(const float *buf, size_t width, size_t height, int channels, int *type);
 
 #if defined(__cplusplus)
 }

@@ -1,5 +1,5 @@
 """Developer micro-benchmark: device-resident timings of the hot-path operators (CUDA events).
-usage: python tools/devbench.py [blur|resize|lab|dilate|erode|gauss|conv2d|stencils|hooks|enhance|layout|all] [size]"""
+usage: python tools/devbench.py [blur|resize|lab|dilate|erode|gauss|conv2d|stencils|hooks|enhance|layout|level|all] [size]"""
 import sys
 from pathlib import Path
 sys.path.insert(0, str(Path(__file__).resolve().parent.parent))
@@ -165,3 +165,34 @@ if which in ("layout", "all"):
         print(f"{name + ' ' + str(size) + '^2':44s} {ms:8.3f} ms  {bpp} B/px  {gbs:7.1f} GB/s  "
               f"{gbs / DATASHEET * 100:5.1f}% of {DATASHEET:.0f} GB/s", flush=True)
     del bufs
+if which in ("level", "all"):
+    # the level and stretch operators at size^2 RGBA, device-resident, with the card and its power limit (part of the
+    # numbers).  Floor: the bytes each operator must move -- a histogram pass reads 16 B/px, an in-place pass reads and
+    # writes 32 B/px, AutoLevel's range pass reads 16 B/px -- at the 3.35 TB/s H100 SXM data-sheet HBM bandwidth.
+    import subprocess
+    DATASHEET = 3350.0
+    try:
+        limit = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i",
+                                str(torch.cuda.current_device())], capture_output=True, text=True, timeout=30).stdout.strip()
+    except (OSError, subprocess.SubprocessError):
+        limit = "unknown"
+    print(f"level operators on {torch.cuda.get_device_name()} at a power limit of {limit or 'unknown'}", flush=True)
+    n = size * size
+    x = im.Image(torch.rand(size, size, 4, device="cuda") * 65535)
+    for name, fn, bpp in [
+            ("LevelImage 1000,60000,1", lambda: im.LevelImage(x, 1000.0, 60000.0, 1.0), 32),
+            ("LevelImage 1000,60000,2.2", lambda: im.LevelImage(x, 1000.0, 60000.0, 2.2), 32),
+            ("LevelizeImage 1000,60000,0.45", lambda: im.LevelizeImage(x, 1000.0, 60000.0, 0.45), 32),
+            ("GammaImage 2.2", lambda: im.GammaImage(x, 2.2), 32),
+            ("AutoLevelImage", lambda: im.AutoLevelImage(x), 48),
+            ("AutoLevelImage -channel RGB", lambda: im.AutoLevelImage(x, 0b0111), 144),
+            ("ContrastStretchImage 1%x97%", lambda: im.ContrastStretchImage(x, 0.01 * n, 0.97 * n), 48),
+            ("NormalizeImage -channel RGBA", lambda: im.NormalizeImage(x, 0b1111), 48),
+            ("LinearStretchImage 2%x1%", lambda: im.LinearStretchImage(x, 0.02 * n, 0.01 * n), 48)]:
+        x.pixels.copy_(torch.rand(size, size, 4, device="cuda") * 65535)
+        ms = timeit(fn, iters=5)
+        gbs = size * size * bpp / ms / 1e6
+        floor = size * size * bpp / DATASHEET / 1e6
+        print(f"{name + ' ' + str(size) + '^2 RGBA':44s} {ms:8.3f} ms  floor {floor:6.3f} ms ({bpp} B/px)  {gbs:7.1f} GB/s  "
+              f"{gbs / DATASHEET * 100:5.1f}% of {DATASHEET:.0f} GB/s", flush=True)
+    del x
