@@ -84,6 +84,7 @@ PROTOTYPES = {
     "mb200_resize_filter_support": (_d, [_i]),
     "mb200_morphology_primitive_dev": (_i, [_vp, _vp, _sz, _sz, _i, _i, KernelPtr, _d, C.POINTER(C.c_longlong), _vp]),
     "mb200_morphology_image_dev": (_i, [_vp, _vp, _sz, _sz, _i, _i, _l, KernelPtr, _d, _vp]),
+    "mb200_morphology_direct_image_dev": (_i, [_vp, _vp, _sz, _sz, _i, _i, KernelPtr, _vp]),
     "mb200_convolve_image_dev": (_i, [_vp, _vp, _sz, _sz, _i, KernelPtr, _vp]),
     "mb200_blur_image_dev": (_i, [_vp, _vp, _sz, _sz, _i, _d, _d, _vp]),
     "mb200_gaussian_blur_image_dev": (_i, [_vp, _vp, _sz, _sz, _i, _d, _d, _vp]),
@@ -97,6 +98,7 @@ PROTOTYPES = {
     "mb200_gaussian_blur_image": (_i, [_vp, _vp, _sz, _sz, _i, _d, _d]),
     "mb200_convolve_image": (_i, [_vp, _vp, _sz, _sz, _i, KernelPtr]),
     "mb200_morphology_image": (_i, [_vp, _vp, _sz, _sz, _i, _i, _l, KernelPtr, _d]),
+    "mb200_morphology_direct_image": (_i, [_vp, _vp, _sz, _sz, _i, _i, KernelPtr]),
     "mb200_unsharp_mask_image": (_i, [_vp, _vp, _sz, _sz, _i, _d, _d, _d, _d]),
     "mb200_resize_image": (_i, [_vp, _sz, _sz, _i, _vp, _sz, _sz, _i]),
     "mb200_transform_colorspace": (_i, [_vp, _sz, _sz, _i, _i, _i]),

@@ -12,6 +12,7 @@ include/magick_b200.h:
     DespeckleImage, LocalContrastImage                              effect.c:1308/2013
     WaveletDenoiseImage                                             visual-effects.c:3515
     MorphologyImage, AcquireKernelInfo                              morphology.c:4129/485
+    MorphologyDirectImage (MorphologyImage: Distance, Voronoi)      morphology.c:3736-3776
     ResizeImage, SampleImage, ScaleImage, ThumbnailImage (pixel)    resize.c:3761/3907/4106/4591
     TransformImageColorspace                                        colorspace.c:1751
     BilevelImage, BlackThresholdImage, WhiteThresholdImage, ClampImage  threshold.c:805/927/2518/1087
@@ -51,6 +52,7 @@ EdgeInMorphology, EdgeOutMorphology, EdgeMorphology, TopHatMorphology, BottomHat
 ErodeIntensityMorphology, DilateIntensityMorphology, IterativeDistanceMorphology = 5, 6, 7
 OpenIntensityMorphology, CloseIntensityMorphology = 10, 11
 HitAndMissMorphology, ThinningMorphology, ThickenMorphology = 18, 19, 20
+DistanceMorphology, VoronoiMorphology = 21, 22
 
 # MagickCore/resample.h:32-69
 (UndefinedFilter, PointFilter, BoxFilter, TriangleFilter, HermiteFilter, HannFilter, HammingFilter,
@@ -223,10 +225,22 @@ def ConvolveImage(image: Image, kernel_info: Union[str, KernelInfo]) -> Image:
 
 def MorphologyImage(image: Image, method: int, iterations: int, kernel: Union[str, KernelInfo],
                     bias: float = 0.0) -> Image:
-    """MagickCore/morphology.c:4129 (bias == the "convolve:bias" artifact)."""
+    """MagickCore/morphology.c:4129 (bias == the "convolve:bias" artifact).  Distance and Voronoi are declined
+    (MB200_EUNSUPPORTED) here; MorphologyDirectImage runs them."""
     k = _as_kernel(kernel)
     return _same_size_op(image, "mb200_morphology_image_dev", "mb200_morphology_image", int(method),
                          int(iterations), k._ptr, float(bias))
+
+
+def MorphologyDirectImage(image: Image, method: int, kernel: Union[str, KernelInfo]) -> Image:
+    """MorphologyImage with DistanceMorphology or VoronoiMorphology (MagickCore/morphology.c:3736-3776): one forward and
+    one reverse sweep with the head kernel of the list -- the reference ignores the iteration count (0 aside) and the
+    bias for these methods.  Voronoi needs an image with alpha (its result takes the source's alpha, and the reference
+    leaves the alpha trait at Copy); on an image without alpha it raises MB200_EUNSUPPORTED, because the reference's
+    result has one channel more."""
+    k = _as_kernel(kernel)
+    return _same_size_op(image, "mb200_morphology_direct_image_dev", "mb200_morphology_direct_image", int(method),
+                         k._ptr)
 
 
 def UnsharpMaskImage(image: Image, radius: float, sigma: float, gain: float, threshold: float) -> Image:

@@ -447,6 +447,28 @@ int mb200_morphology_image_dev(const float *src, float *dst, size_t width, size_
   return morphology_apply(src, dst, width, height, channels, method, iterations, kernel, bias, s);
 }
 
+// Distance / Voronoi: the arguments are checked before the device; forward pass into a pool temporary, reverse into dst.
+static int morphology_direct_args(const float *src, const float *dst, size_t width, size_t height, int channels,
+                                  int method, const mb200_kernel_info *kernel) {
+  if (!src || !dst || src == dst || !valid_image(width, height, channels))
+    return fail(MB200_EINVAL, "morphology direct: bad arguments");
+  if (width > (1u << 30) || height > (1u << 30))
+    return fail(MB200_EUNSUPPORTED, "morphology direct: images wider or taller than 2^30 are not supported");
+  return morphology_direct_check(channels, method, kernel);
+}
+
+int mb200_morphology_direct_image_dev(const float *src, float *dst, size_t width, size_t height, int channels,
+                                      int method, const mb200_kernel_info *kernel, void *stream) {
+  int rc = morphology_direct_args(src, dst, width, height, channels, method, kernel);
+  cudaStream_t s;
+  if (!rc) rc = prepare(stream, &s);
+  if (rc) return rc;
+  StreamAlloc tmp(s);
+  rc = tmp.alloc(image_bytes(width, height, channels));
+  if (rc) return rc;
+  return launch_morphology_direct(src, static_cast<float *>(tmp.ptr), dst, width, height, channels, method, kernel, s);
+}
+
 int mb200_convolve_image_dev(const float *src, float *dst, size_t width, size_t height, int channels,
                              const mb200_kernel_info *kernel, void *stream) {
   return mb200_morphology_image_dev(src, dst, width, height, channels, MB200_ConvolveMorphology, 1, kernel, 0.0,
@@ -613,6 +635,15 @@ int mb200_morphology_image(const float *src, float *dst, size_t w, size_t h, int
   if (!kernel) return fail(MB200_EINVAL, "morphology: bad arguments");
   return with_staging("morphology", src, w, h, ch, dst, w, h, [&](const float *s, float *d, cudaStream_t st) {
     return mb200_morphology_image_dev(s, d, w, h, ch, method, iterations, kernel, bias, st);
+  });
+}
+
+int mb200_morphology_direct_image(const float *src, float *dst, size_t w, size_t h, int ch, int method,
+                                  const mb200_kernel_info *kernel) {
+  const int rc = morphology_direct_args(src, dst, w, h, ch, method, kernel);
+  if (rc) return rc;
+  return with_staging("morphology direct", src, w, h, ch, dst, w, h, [&](const float *s, float *d, cudaStream_t st) {
+    return mb200_morphology_direct_image_dev(s, d, w, h, ch, method, kernel, st);
   });
 }
 

@@ -40,6 +40,7 @@ enum LaunchFamily {
   kResizeRegular, kResizeGather,                                       // resize.cu
   kConv2dDenseR8, kConv2dDenseR4, kConv2dDenseR2, kMorph2d, kMinmax2d, // morph2d.cu
   kMorphStream,                                                        // morph_stream.cu
+  kMorphDirect,                                                        // morph_direct.cu
   kLaunchFamilies
 };
 void count_family(LaunchFamily family);
@@ -116,6 +117,14 @@ int launch_morph2d(const float *src, float *dst, size_t width, size_t height, in
 // (MB200_EUNSUPPORTED => shape not in the table; use launch_morph2d)
 int launch_morph_stream(const float *src, float *dst, size_t width, size_t height, int channels, int method,
                         const double *kernel_window_order, int kw, int kh, int ox, int oy, void *stream);
+
+// morph_direct.cu: MorphologyApply's Distance / Voronoi branch (the two sequential sweeps of MorphologyPrimitiveDirect
+// and Voronoi's alpha epilogue).  The check runs on the host before anything is allocated (MB200_EINVAL: another method,
+// no kernel, an origin outside it; MB200_EUNSUPPORTED: Voronoi without alpha, a kernel too large for the wavefront);
+// the launcher takes a temporary of the image's size for the forward pass.
+int morphology_direct_check(int channels, int method, const mb200_kernel_info *kernel);
+int launch_morphology_direct(const float *src, float *tmp, float *dst, size_t width, size_t height, int channels,
+                             int method, const mb200_kernel_info *kernel, void *stream);
 
 // ---- resize axis tables (resize_tables.cpp) ---------------------------------
 // One axis of ResizeImage, planned on the host and resident on one device: the reference's contribution lists

@@ -277,6 +277,40 @@ static int op_morphology(const float *s, float *d, size_t w, size_t h, int ch, c
   return rc;
 }
 
+/* Distance / Voronoi (morphology.c:3736-3776): one run of MorphologyPrimitiveDirect with the head kernel of the list,
+   whatever the iteration count (0 aside) and bias. */
+typedef struct { int method; const KernelInfo *kernel; } direct_args;
+static int op_morphology_direct(const float *s, float *d, size_t w, size_t h, int ch, const void *a)
+{
+  const direct_args *m = (const direct_args *) a;
+  mb200_kernel_info node;
+  memset(&node, 0, sizeof(node));
+  node.type = map_kernel_type(m->kernel->type);
+  node.width = m->kernel->width; node.height = m->kernel->height;
+  node.x = (long) m->kernel->x; node.y = (long) m->kernel->y;
+  node.values = (double *) m->kernel->values;    /* MagickRealType == double; read-only use */
+  return mb200_morphology_direct_image(s, d, w, h, ch, m->method, &node);
+}
+
+static Image *morphology_direct(const Image *image, const MorphologyMethod method, const KernelInfo *kernel,
+                                ExceptionInfo *exception)
+{
+  direct_args a;
+  Image *out;
+  a.method = (int) method; a.kernel = kernel;
+  if (method == DistanceMorphology)
+    /* Copy-trait channels are skipped by the sweeps and so keep the clone's value: the restore pass gives the same */
+    return run_same_size_masked(image, op_morphology_direct, &a, 1, exception);
+  /* Voronoi ends in SetImageAlphaChannel(Deactivate), CompositeImage(CopyAlpha), Deactivate (:3766-3774).  The library
+     computes the composite's result for the default compose settings and traits on an image with alpha; without alpha
+     the result gains a channel, and a -channel selection would change what the composite writes. */
+  if (image->alpha_trait == UndefinedPixelTrait) return (Image *) NULL;
+  if (has_artifact(image, compose_artifacts) != MagickFalse) return (Image *) NULL;
+  out = run_same_size_masked(image, op_morphology_direct, &a, 0, exception);
+  if (out != (Image *) NULL) (void) SetImageAlphaChannel(out, DeactivateAlphaChannel, exception);   /* Blend -> Copy */
+  return out;
+}
+
 Image *B200AccelerateMorphologyImage(const Image *image, const MorphologyMethod method,
                                      const ssize_t iterations, const KernelInfo *kernel,
                                      ExceptionInfo *exception)
@@ -326,7 +360,8 @@ Image *B200AccelerateMorphologyImage(const Image *image, const MorphologyMethod 
         allow_mask = 0;
       }
       break;
-    default: return (Image *) NULL;          /* Distance / Voronoi: sequential two-pass primitives stay on the CPU */
+    case DistanceMorphology: case VoronoiMorphology: return morphology_direct(image, method, kernel, exception);
+    default: return (Image *) NULL;
   }
   a.method = (int) method; a.iterations = (long) iterations; a.kernel = scaled != (KernelInfo *) NULL ? scaled : kernel;
   out = run_same_size_masked(image, op_morphology, &a, allow_mask, exception);

@@ -237,6 +237,36 @@ int main(void)
   k = AcquireKernelInfo("Euclidean:2", ex);
   CHECK("MorphologyImage IterativeDistance x4", 0, MorphologyImage(rgb, IterativeDistanceMorphology, 4, k, ex), CPU(__real_MorphologyImage(rgb, IterativeDistanceMorphology, 4, k, ex)));
   k = DestroyKernelInfo(k);
+  {
+    /* Distance / Voronoi (MorphologyPrimitiveDirect): one run of the head kernel.  Voronoi leaves the alpha trait at
+       Copy, and on an image without alpha (whose result gains an alpha channel) it must decline and still be right. */
+    const long hits0 = B200ShimHits();
+    Image *ga = converted(rgba, GRAYColorspace, ex);
+    long fb;
+    k = AcquireKernelInfo("Euclidean:4", ex);
+    CHECK("MorphologyImage Distance Euclidean:4 RGBA", 0, MorphologyImage(rgba, DistanceMorphology, 1, k, ex), CPU(__real_MorphologyImage(rgba, DistanceMorphology, 1, k, ex)));
+    CHECK("MorphologyImage Distance Euclidean:4 GA", 0, MorphologyImage(ga, DistanceMorphology, 3, k, ex), CPU(__real_MorphologyImage(ga, DistanceMorphology, 3, k, ex)));
+    (void) SetPixelChannelMask(rgba, (ChannelType) (RedChannel | BlueChannel | AlphaChannel));
+    CHECK("MorphologyImage Distance -channel RBA", 0, MorphologyImage(rgba, DistanceMorphology, 1, k, ex), CPU(__real_MorphologyImage(rgba, DistanceMorphology, 1, k, ex)));
+    (void) SetPixelChannelMask(rgba, DefaultChannels);
+    k = DestroyKernelInfo(k);
+    k = AcquireKernelInfo("Chebyshev:2", ex);
+    a = MorphologyImage(rgba, VoronoiMorphology, 1, k, ex); b = CPU(__real_MorphologyImage(rgba, VoronoiMorphology, 1, k, ex));
+    if (!a || !b || a->alpha_trait != b->alpha_trait || GetPixelChannels(a) != GetPixelChannels(b)) {
+      printf("MorphologyImage Voronoi RGBA: alpha trait / channels differ  FAIL\n"); failures++;
+    }
+    CHECK("MorphologyImage Voronoi Chebyshev:2 RGBA", 0, a, b);
+    fb = B200ShimFallbacks();
+    a = MorphologyImage(rgb, VoronoiMorphology, 1, k, ex); b = CPU(__real_MorphologyImage(rgb, VoronoiMorphology, 1, k, ex));
+    if (!a || !b || a->alpha_trait != b->alpha_trait || GetPixelChannels(a) != GetPixelChannels(b)) {
+      printf("MorphologyImage Voronoi RGB: alpha trait / channels differ  FAIL\n"); failures++;
+    }
+    CHECK("MorphologyImage Voronoi RGB (declines)", 0, a, b);
+    if (mb200_device_count() > 0 && B200ShimFallbacks() <= fb) { printf("FAIL: Voronoi without alpha was not declined\n"); failures++; }
+    if (mb200_device_count() > 0 && B200ShimHits() - hits0 < 4) { printf("FAIL: Distance / Voronoi did not reach the GPU path\n"); failures++; }
+    k = DestroyKernelInfo(k);
+    ga = DestroyImage(ga);
+  }
   a = CloneImage(rgba, 0, 0, MagickTrue, ex); b = CloneImage(rgba, 0, 0, MagickTrue, ex);
   if (TransformImageColorspace(a, LabColorspace, ex) == MagickFalse || a->colorspace != LabColorspace) failures++;
   B200ShimEnable(0); (void) __real_TransformImageColorspace(b, LabColorspace, ex); B200ShimEnable(1);

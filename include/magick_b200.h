@@ -69,7 +69,9 @@ typedef enum {
   MB200_BottomHatMorphology = 17,
   MB200_HitAndMissMorphology = 18,
   MB200_ThinningMorphology = 19,
-  MB200_ThickenMorphology = 20
+  MB200_ThickenMorphology = 20,
+  MB200_DistanceMorphology = 21,
+  MB200_VoronoiMorphology = 22
 } mb200_morphology_method;
 
 /* MagickCore/resample.h:32-69 FilterType -- same numeric values */
@@ -315,10 +317,23 @@ MB200_API int mb200_morphology_primitive_dev(const float *src, float *dst, size_
    "difference" methods EdgeIn / EdgeOut / Edge / TopHat / BottomHat, whose final
    CompositeImage(..., DifferenceCompositeOp, ...) step (:3995-4012) runs as one point
    kernel (bit exact).  HitAndMiss / Thinning / Thicken / Distance / Voronoi / the
-   *Intensity methods return MB200_EUNSUPPORTED. */
+   *Intensity methods return MB200_EUNSUPPORTED; Distance and Voronoi have their own
+   entry point, mb200_morphology_direct_image_dev. */
 MB200_API int mb200_morphology_image_dev(const float *src, float *dst, size_t width,
     size_t height, int channels, int method, long iterations,
     const mb200_kernel_info *kernel, double bias, void *stream);
+
+/* MorphologyImage with the directly applied methods, Distance and Voronoi (MagickCore/morphology.c:3736-3776,
+   MorphologyPrimitiveDirect :3242-3623): one forward and one reverse sweep, whatever the iteration count and bias, with
+   the head kernel of the list only.  Bit exact.  Every channel is swept (a `-channel` selection is put back with
+   mb200_restore_channels_dev).  Voronoi replaces the swept alpha with the source's, ClampPixel(QuantumRange*QuantumScale*a),
+   clamps the other channels to [0, QuantumRange], and leaves the image's alpha trait at Copy (the caller's to record);
+   on an image without alpha its result needs one more channel, so it returns MB200_EUNSUPPORTED.  MB200_EINVAL: a method
+   other than Distance / Voronoi, no kernel, or an origin outside the kernel; MB200_EUNSUPPORTED also for kernels the
+   wavefront cannot hold (more than 1 024 non-NaN cells in a pass, more than 32 rows on one side of the origin, or rings
+   beyond shared memory).  Both are checked before the device is touched. */
+MB200_API int mb200_morphology_direct_image_dev(const float *src, float *dst, size_t width, size_t height,
+    int channels, int method, const mb200_kernel_info *kernel, void *stream);
 
 /* ConvolveImage (MagickCore/effect.c:1170) */
 MB200_API int mb200_convolve_image_dev(const float *src, float *dst, size_t width, size_t height,
@@ -573,6 +588,8 @@ MB200_API int mb200_convolve_image(const float *src, float *dst, size_t width, s
     int channels, const mb200_kernel_info *kernel);
 MB200_API int mb200_morphology_image(const float *src, float *dst, size_t width, size_t height,
     int channels, int method, long iterations, const mb200_kernel_info *kernel, double bias);
+MB200_API int mb200_morphology_direct_image(const float *src, float *dst, size_t width, size_t height,
+    int channels, int method, const mb200_kernel_info *kernel);
 MB200_API int mb200_unsharp_mask_image(const float *src, float *dst, size_t width, size_t height,
     int channels, double radius, double sigma, double gain, double threshold);
 MB200_API int mb200_sharpen_image(const float *src, float *dst, size_t width, size_t height, int channels,

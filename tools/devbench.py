@@ -1,5 +1,5 @@
 """Developer micro-benchmark: device-resident timings of the hot-path operators (CUDA events).
-usage: python tools/devbench.py [blur|resize|lab|dilate|erode|gauss|conv2d|stencils|hooks|enhance|layout|level|all] [size]"""
+usage: python tools/devbench.py [blur|resize|lab|dilate|erode|gauss|conv2d|stencils|hooks|enhance|layout|level|direct|all] [size]"""
 import sys
 from pathlib import Path
 sys.path.insert(0, str(Path(__file__).resolve().parent.parent))
@@ -195,4 +195,46 @@ if which in ("level", "all"):
         floor = size * size * bpp / DATASHEET / 1e6
         print(f"{name + ' ' + str(size) + '^2 RGBA':44s} {ms:8.3f} ms  floor {floor:6.3f} ms ({bpp} B/px)  {gbs:7.1f} GB/s  "
               f"{gbs / DATASHEET * 100:5.1f}% of {DATASHEET:.0f} GB/s", flush=True)
+    del x
+if which in ("direct", "all"):
+    # Distance / Voronoi morphology at size^2 RGBA, device-resident, with the card and its power limit.  Floor: two
+    # passes of 16 B/px read + 16 B/px written (64 B/px) at the 3.35 TB/s H100 SXM data-sheet HBM bandwidth.  Critical
+    # path: wavefront steps of the two passes, (rows-1)*skew + columns each (skew = reach right + 1).  Where
+    # oracle/_ref is built, the reference's own MorphologyImage runs single-threaded on the same image.
+    import ctypes
+    import subprocess
+    import time
+    import numpy as np
+    DATASHEET = 3350.0
+    try:
+        limit = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i",
+                                str(torch.cuda.current_device())], capture_output=True, text=True, timeout=30).stdout.strip()
+    except (OSError, subprocess.SubprocessError):
+        limit = "unknown"
+    print(f"Distance / Voronoi on {torch.cuda.get_device_name()} at a power limit of {limit or 'unknown'}", flush=True)
+    ref_so = Path(__file__).resolve().parent.parent / "oracle" / "_ref" / "libmagickref_direct.so"
+    ref = ctypes.CDLL(str(ref_so)) if ref_so.exists() else None
+    src = (torch.rand(size, size, 4, device="cuda") > 0.02).float() * 65535
+    x = im.Image(src)
+    host = src.cpu().numpy()
+    floor = size * size * 64 / DATASHEET / 1e6
+    for method, kernel in [(im.DistanceMorphology, "Euclidean"), (im.DistanceMorphology, "Euclidean:4"),
+                           (im.DistanceMorphology, "Chebyshev:2"), (im.VoronoiMorphology, "Euclidean")]:
+        vals, kx, ky = im.AcquireKernelInfo(kernel).arrays()[0]
+        kh, kw = vals.shape
+        steps = (size - 1) * (kx + 1) + size + (size - 1) * (kw - kx) + size
+        ms = timeit(lambda: im.MorphologyDirectImage(x, method, kernel), iters=5)
+        name = ("Distance " if method == im.DistanceMorphology else "Voronoi ") + kernel
+        line = (f"{name + ' ' + str(size) + '^2 RGBA':36s} {ms:9.3f} ms  floor {floor:5.3f} ms = {floor / ms * 100:5.2f}%  "
+                f"critical path {steps} steps ({ms * 1e6 / steps:6.1f} ns/step)")
+        if ref is not None:
+            ref.ref_set_threads(1)
+            out = np.empty((size, size, 5), np.float32)
+            trait = ctypes.c_int()
+            t0 = time.perf_counter()
+            rc = ref.ref_morphology_direct(ctypes.c_void_p(host.ctypes.data), ctypes.c_void_p(out.ctypes.data), ctypes.c_size_t(size), ctypes.c_size_t(size),
+                                           4, method, ctypes.c_long(1), ctypes.c_char_p(kernel.encode()), ctypes.byref(trait))
+            t = time.perf_counter() - t0
+            line += f"  reference 1 thread {t * 1e3:9.1f} ms (rc {rc})"
+        print(line, flush=True)
     del x
