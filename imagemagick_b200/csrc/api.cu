@@ -554,11 +554,13 @@ int mb200_resize_image_ex_dev(const float *src, size_t width, size_t height, int
     return launch_resize_axis(in, w, h, channels, out, axis, t, axis == 1 || knobs.resize_regular_h, s);
   };
   // Equal integer reduction on both axes (the reference filters vertically first when x_factor <= y_factor, :3854-3861):
-  // one fused launch keeps the vertically filtered intermediate of every output tile in shared memory.  Parity-green and
-  // bit-identical to the two passes, DRAM traffic 1.32 GB instead of 2.45 GB for 8192^2 -> 4096^2 -- but slower: the
-  // passes are bound by the FP64 and conversion (XU) pipes, not by HBM, and the fused kernel adds 17 % of halo work.
-  // Opt-in (MB200_RESIZE_FUSED=1 / mb200_set_option("resize_fused", 1)).
-  if (channels == 4 && c.x_factor == c.y_factor && !knobs.no_resize_stream && knobs.resize_fused) {
+  // one fused launch keeps the vertically filtered intermediate of every output tile in shared memory, with the same
+  // bits as the two passes.  It moves 20 B per source pixel through HBM instead of 36, which pays once the two-pass
+  // intermediate no longer stays in L2; below that the two passes' extra traffic never leaves the chip and they are
+  // faster (DESIGN §5.4).
+  const bool big = width * out_height * px > l2_bytes();
+  if (channels == 4 && c.x_factor == c.y_factor && !knobs.no_resize_stream && !knobs.no_resize_fused &&
+      (knobs.resize_fused || big)) {
     rc = launch_resize_fused(src, width, height, dst, *tx, *ty, s);
     if (rc != MB200_EUNSUPPORTED) return rc;
   }

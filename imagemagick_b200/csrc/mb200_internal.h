@@ -27,7 +27,8 @@ struct TuningKnobs {
   int pair, pair_async, pair_async_col, col_rot, row_pair_rot, row_rot;   // conv1d.cu
   int resize_tma, resize_chunk, resize_slots, resize_strip;           // resize_stream.cu
   // switches (0 / 1) that force the generic paths, or opt in to a slower one, in api.cu
-  int no_rank1, no_morph_stream, no_resize_stream, resize_regular_h, no_fused_unsharp, resize_fused;
+  int no_rank1, no_morph_stream, no_resize_stream, resize_regular_h, no_fused_unsharp;
+  int resize_fused, no_resize_fused;                                   // force the fused / the two-pass ResizeImage
   int conv2d_rows;                                                     // morph2d.cu: 0 automatic, else 8 / 4 / 2
 };
 TuningKnobs tuning_knobs();
@@ -36,7 +37,7 @@ TuningKnobs tuning_knobs();
 enum LaunchFamily {
   kConvMma,                                                            // conv_mma.cu
   kConvPair, kConvPairAsync, kConvGeneric,                             // conv1d.cu
-  kResizeVStream, kResizeHTma, kResizeHStream,                         // resize_stream.cu
+  kResizeVStream, kResizeHTma, kResizeHStream, kResizeFused,           // resize_stream.cu
   kResizeRegular, kResizeGather,                                       // resize.cu
   kConv2dDenseR8, kConv2dDenseR4, kConv2dDenseR2, kMorph2d, kMinmax2d, // morph2d.cu
   kMorphStream,                                                        // morph_stream.cu
@@ -51,6 +52,7 @@ int ensure_device();                     // lazily initialises the current devic
 void *default_stream();                  // library-owned stream of the current device
 int scratch(void **ptr, size_t bytes, int slot);   // grow-only device scratch buffers
 int sm_count();
+size_t l2_bytes();                       // L2 cache size of the current device (cudaDevAttrL2CacheSize)
 // The library's PRIVATE stream-ordered memory pool of the current device (temporaries of the operators).  The host
 // application's default pool is left alone; mb200_trim() gives the cached memory back.
 ::CUmemPoolHandle_st *temp_pool();

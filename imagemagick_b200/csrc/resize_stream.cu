@@ -485,11 +485,29 @@ struct FusedArgs {
   const double *wx, *wy;        // [run][N] weights
 };
 
+// Phase B of warp w reads the tile row from sample S*NW*w up to niter*BODY + 1 samples further: inside the 128 columns
+// phase A filled for the last warp, whose source span S*(4*NW-1)+N must itself fit them.
+template <int S, int N>
+constexpr bool fused_fits(int nw) {
+  return S * (4 * nw - 1) + N <= 128 &&
+         S * 3 * nw + ((S * (nw - 1) + N + Rot<S, N>::BODY - 1) / Rot<S, N>::BODY) * Rot<S, N>::BODY + 1 <= 128;
+}
+template <int S, int N>
+constexpr int fused_nw() {
+  int nw = 13;
+  while (nw > 1 && !fused_fits<S, N>(nw)) --nw;
+  return nw;
+}
+
 template <int S, int N> struct FusedGeom {
   static constexpr int P = Rot<S, N>::P;
   static constexpr int TH = 31;                                  // S*(TH-1)+N = 72 = 6*P for S=2, N=12
-  static constexpr int NW = (128 - N) / S / 4 >= 13 ? 13 : (128 - N) / S / 4;   // S*(4*NW-1)+N <= 128
+  static constexpr int NW = fused_nw<S, N>();                    // output columns per warp in phase B
+  static_assert(fused_fits<S, N>(NW), "no phase-B split fits the 128-column tile");
   static constexpr int TW = 4 * NW;
+  // phase-A prefetch depth: the vertical kernel's, except (2,12), whose 12-deep ring spills at 168 registers (3 CTAs / SM);
+  // 6 loads of 16 B per thread still keep ~36 KB per SM in flight
+  static constexpr int PF = Rot<S, N>::PF == 12 ? 6 : Rot<S, N>::PF;
   static constexpr int kPitch = 128 * 16 + 16;                   // bytes per tile row
   static constexpr int kSmem = 32 * kPitch;
 };
@@ -498,7 +516,7 @@ template <int S, int N>
 __global__ void __launch_bounds__(128, 3) resize_fused_kernel(const FusedArgs a) {
   using T = Rot<S, N>;
   using G = FusedGeom<S, N>;
-  constexpr int R = T::R, P = T::P, BODY = T::BODY, PF = T::PF;
+  constexpr int R = T::R, P = T::P, BODY = T::BODY, PF = G::PF;
   extern __shared__ __align__(16) unsigned char inter[];        // [TH][kPitch]
   const Tile xt = a.xt[blockIdx.x], yt = a.yt[blockIdx.y];
   double acc[R][4];
@@ -549,9 +567,7 @@ __global__ void __launch_bounds__(128, 3) resize_fused_kernel(const FusedArgs a)
     double W[N];
 #pragma unroll
     for (int j = 0; j < N; ++j) W[j] = __ldg(a.wx + xt.set * N + j);
-    const int niter = (S * (nout - 1) + N + BODY - 1) / BODY;
-    // the last warp reads S*3*NW + niter*BODY + 1 <= 128 samples of its row: never past the tile
-    static_assert(S * 3 * G::NW + ((S * (G::NW - 1) + N + BODY - 1) / BODY) * BODY + 1 <= 128, "phase B would leave the tile row");
+    const int niter = (S * (nout - 1) + N + BODY - 1) / BODY;   // the last warp never reads past the tile (fused_fits)
     const unsigned char *rd = inter + static_cast<size_t>(lane) * G::kPitch + static_cast<size_t>(S * o_first) * 16;
 #pragma unroll
     for (int q = 0; q < R; ++q) { acc[q][0] = acc[q][1] = acc[q][2] = acc[q][3] = 0.0; }
@@ -648,8 +664,13 @@ int launch_fused_sn(const FusedArgs &a, int nxt, int nyt, cudaStream_t s) {
 // Tile geometry of the fused kernel for (stride, taps): outputs per tile along x / y; 0 = no fused kernel for this pair.
 void resize_fused_tile(int stride, int taps, int *tw, int *th) {
   *tw = *th = 0;
-  if (stride == 2 && taps == 12) { *tw = FusedGeom<2, 12>::TW; *th = FusedGeom<2, 12>::TH; }
-  else if (stride == 2 && taps == 8) { *tw = FusedGeom<2, 8>::TW; *th = FusedGeom<2, 8>::TH; }
+  auto set = [&](auto geom) { *tw = decltype(geom)::TW; *th = decltype(geom)::TH; };
+  if (stride == 2 && taps == 12) set(FusedGeom<2, 12>{});
+  else if (stride == 2 && taps == 8) set(FusedGeom<2, 8>{});
+  else if (stride == 2 && taps == 4) set(FusedGeom<2, 4>{});
+  else if (stride == 3 && taps == 19) set(FusedGeom<3, 19>{});
+  else if (stride == 4 && taps == 24) set(FusedGeom<4, 24>{});
+  else if (stride == 4 && taps == 16) set(FusedGeom<4, 16>{});
 }
 
 // Fused vertical + horizontal pass: the tiles of both axes' runs, then the two-pass path's contribution and border lists
@@ -670,8 +691,13 @@ int launch_resize_fused(const float *src, size_t width, size_t height, float *ds
   int rc = MB200_EUNSUPPORTED;
   if (stride == 2 && taps == 12) rc = launch_fused_sn<2, 12>(a, nxt, nyt, s);
   else if (stride == 2 && taps == 8) rc = launch_fused_sn<2, 8>(a, nxt, nyt, s);
+  else if (stride == 2 && taps == 4) rc = launch_fused_sn<2, 4>(a, nxt, nyt, s);
+  else if (stride == 3 && taps == 19) rc = launch_fused_sn<3, 19>(a, nxt, nyt, s);
+  else if (stride == 4 && taps == 24) rc = launch_fused_sn<4, 24>(a, nxt, nyt, s);
+  else if (stride == 4 && taps == 16) rc = launch_fused_sn<4, 16>(a, nxt, nyt, s);
   if (rc != MB200_OK) return rc;
   count_launch();
+  count_family(kResizeFused);
   if (x.nborder > 0 || y.nborder > 0) {
     Border2dArgs b{};
     b.src = src; b.dst = dst; b.width = a.width; b.height = a.height; b.out_w = a.out_w; b.out_h = a.out_h;

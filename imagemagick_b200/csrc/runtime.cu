@@ -31,6 +31,7 @@ struct DeviceStateImpl {
   cudaStream_t stream = nullptr;
   cudaMemPool_t pool = nullptr;      // private pool of the operators' temporaries
   int sms = 0;
+  int l2_bytes = 0;
   void *scratch[kScratchSlots] = {nullptr};
   size_t scratch_bytes[kScratchSlots] = {0};
 };
@@ -97,8 +98,10 @@ const KnobSpec kKnobs[] = {
     {"no_morph_stream", &TuningKnobs::no_morph_stream, 0, any_value, kSwitch},
     {"no_resize_stream", &TuningKnobs::no_resize_stream, 0, any_value, kSwitch},
     {"no_fused_unsharp", &TuningKnobs::no_fused_unsharp, 0, any_value, kSwitch},
-    // opt-in paths that measured slower than the defaults
+    {"no_resize_fused", &TuningKnobs::no_resize_fused, 0, any_value, kSwitch},
+    // opt-in path that measured slower than the default
     {"resize_regular_h", &TuningKnobs::resize_regular_h, 0, any_value, kSwitch},
+    // the fused ResizeImage wherever it applies, also below the automatic size threshold
     {"resize_fused", &TuningKnobs::resize_fused, 0, any_value, kSwitch},
 };
 constexpr size_t kNumKnobs = sizeof(kKnobs) / sizeof(kKnobs[0]);
@@ -136,9 +139,9 @@ int knob_index(const char *name) {
 
 const char *const kFamilyNames[kLaunchFamilies] = {
     "conv_mma_launches", "conv_pair_launches", "conv_pair_async_launches", "conv_generic_launches",
-    "resize_v_stream_launches", "resize_h_tma_launches", "resize_h_stream_launches", "resize_regular_launches",
-    "resize_gather_launches", "conv2d_dense_r8_launches", "conv2d_dense_r4_launches", "conv2d_dense_r2_launches",
-    "morph2d_launches", "minmax2d_launches", "morph_stream_launches", "morph_direct_launches"};
+    "resize_v_stream_launches", "resize_h_tma_launches", "resize_h_stream_launches", "resize_fused_launches",
+    "resize_regular_launches", "resize_gather_launches", "conv2d_dense_r8_launches", "conv2d_dense_r4_launches",
+    "conv2d_dense_r2_launches", "morph2d_launches", "minmax2d_launches", "morph_stream_launches", "morph_direct_launches"};
 std::atomic<unsigned long long> g_family_launches[kLaunchFamilies];
 int family_index(const char *name) {
   for (int f = 0; f < kLaunchFamilies; ++f)
@@ -171,6 +174,8 @@ int ensure_device() {
     return fail(MB200_ENODEVICE, "device %d is sm_%d%d; libmagickb200 carries sm_90a code only", dev,
                 prop.major, prop.minor);
   d.sms = prop.multiProcessorCount;
+  e = cudaDeviceGetAttribute(&d.l2_bytes, cudaDevAttrL2CacheSize, dev);
+  if (e != cudaSuccess) return cuda_fail(e, "cudaDeviceGetAttribute(L2 size)");
   e = cudaStreamCreateWithFlags(&d.stream, cudaStreamNonBlocking);
   if (e != cudaSuccess) return cuda_fail(e, "cudaStreamCreate");
   {
@@ -219,6 +224,11 @@ void *default_stream() {
 int sm_count() {
   DeviceStateImpl *d = current();
   return d && d->sms ? d->sms : 132;
+}
+
+size_t l2_bytes() {
+  DeviceStateImpl *d = current();
+  return d && d->l2_bytes > 0 ? static_cast<size_t>(d->l2_bytes) : size_t{50} << 20;
 }
 
 int scratch(void **ptr, size_t bytes, int slot) {

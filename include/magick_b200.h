@@ -192,7 +192,9 @@ MB200_API int mb200_trim(size_t keep_bytes);
    the co-limit of the FP64-accumulating convolution kernels (bench.py's second roofline entry). */
 MB200_API int mb200_probe_fp64_fma_rate(double *fma_per_second);
 /* Test / developer hook: force the generic kernels ("no_rank1", "no_morph_stream", "no_resize_stream",
-   "resize_regular_h", "no_fused_unsharp", "resize_fused", "conv_mma" = the FP64 mma.sync kernels of conv_mma.cu for
+   "resize_regular_h", "no_fused_unsharp", "no_resize_fused" = the two streaming passes of ResizeImage where the fused
+   vertical + horizontal kernel would run, "resize_fused" = that kernel wherever it applies, also on images whose two-pass
+   intermediate fits in L2, "conv_mma" = the FP64 mma.sync kernels of conv_mma.cu for
    RGBA 1-D passes: 1 whenever possible, 0 never, -1 automatic = float-in / float-out passes; initialised from the MB200_<NAME> environment variables).  mb200_get_option reads a switch back;
    "conv_mma_launches" counts the passes the mma.sync kernels have served since process start.
    The tuning knobs of DESIGN §10 are options too: "mma_strip" (>= 8, rounded up to a multiple of 8), "mma_minb" (3, 4),
@@ -201,7 +203,8 @@ MB200_API int mb200_probe_fp64_fma_rate(double *fma_per_second);
    (>= 0); the counts go up to 2^20.  Any other value is rejected with MB200_EINVAL (an invalid environment value is
    ignored: the default applies).  Launch counters per kernel family, readable like "conv_mma_launches":
    "conv_pair_launches", "conv_pair_async_launches", "conv_generic_launches", "resize_v_stream_launches",
-   "resize_h_tma_launches", "resize_h_stream_launches", "resize_regular_launches", "resize_gather_launches". */
+   "resize_h_tma_launches", "resize_h_stream_launches", "resize_fused_launches", "resize_regular_launches",
+   "resize_gather_launches". */
 MB200_API int mb200_set_option(const char *name, int value);
 MB200_API int mb200_get_option(const char *name, int *value);
 
