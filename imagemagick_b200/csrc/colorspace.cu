@@ -35,7 +35,12 @@ namespace {
 // arithmetic (15 instructions per channel) disappears from a kernel that ncu shows to be issue-bound.
 __constant__ double kDecodeScale[128];
 
-__device__ __noinline__ double decode_gamma_far(double x) { return decode_gamma(x); }
+// +inf settles like the reference's frexp / Chebyshev chain: NaN (decode_gamma's exponent-field frexp assumes a finite
+// argument; a NaN argument stays NaN through its final product)
+__device__ __noinline__ double decode_gamma_far(double x) {
+  if (!(x <= 1.7976931348623157e308)) return __longlong_as_double(0x7ff8000000000000LL);
+  return decode_gamma(x);
+}
 
 __device__ __forceinline__ double decode_gamma_tab(double x, const double *s_scale) {
   const int hi = __double2hiint(x);
@@ -67,13 +72,15 @@ __device__ __forceinline__ void rgb_to_xyz(double R, double G, double B, double 
 // cancels there, and a black pixel must give exactly 0, not -1e-13 (a huge ULP distance for a very common value).
 // The fast path is straight-line code (no divergent region per channel: the three Horner chains interleave and the
 // BSSY / BSYNC / BRA scaffolding of six conditionals disappears): the toe is a select, and the two rare cases -- an
-// HDRI sample whose gamma argument leaves the tabled exponents, a Lab argument below the CIE epsilon -- are collected
-// into one flag each and handled per pixel by out-of-line code.
+// HDRI sample whose gamma argument leaves the tabled exponents (or is +inf / NaN), a Lab argument below the CIE epsilon
+// or at or above 2 (cube_root5's range) -- are collected into one flag each and handled per pixel by out-of-line code.
 // (toe test in float: for a float sample p, (double)p <= 0.0404482362771076*QuantumRange  <=>  p <= 2650.775146484375f,
 // the largest float below that limit; the Lab test on the high words: positive doubles order like their bit patterns,
-// and anything at or below the word of the CIE epsilon -- or negative -- takes the exact out-of-line code.)
+// and anything at or below the word of the CIE epsilon -- or negative -- or with the top exponent bit set (2 and above,
+// +inf, NaN) takes the exact out-of-line code.)
 constexpr float kToeLimitF = 2650.775146484375f;
 constexpr int kCieEpsHi = 0x3f822354;          // high word of 216/24389 = 0x3f822354d28f7cd6
+constexpr int kTwoAndAboveBit = 0x40000000;    // the top exponent bit of a high word (kCubeRootSeedMax = 2)
 __device__ __forceinline__ double decode_unit(float sample, const double *s_scale, bool &far) {   // QuantumScale * DecodePixelGamma
   const double pixel = static_cast<double>(sample);
   const double x = fma(pixel, kk.slope_unit, kk.offset_unit);
@@ -88,10 +95,11 @@ __device__ __forceinline__ double decode_unit(float sample, const double *s_scal
 }
 __device__ __noinline__ double decode_unit_far(double pixel) {
   if (pixel <= kk.toe_limit) return pixel * kk.toe_unit;
+  if (!(pixel <= 1.7976931348623157e308)) return __longlong_as_double(0x7ff8000000000000LL);   // as decode_gamma_far
   return decode_gamma(fma(pixel, kk.slope_unit, kk.offset_unit));
 }
 __device__ __noinline__ double lab_f_toe(double t) {
-  if (t > kk.cie_eps) return cube_root5(t);
+  if (t > kk.cie_eps) return cube_root(t);
   return (kCieK * t + 16.0) / 116.0;
 }
 __device__ __forceinline__ void rgb_to_lab_unit(float R, float G, float B, double &o0, double &o1, double &o2,
@@ -103,7 +111,10 @@ __device__ __forceinline__ void rgb_to_lab_unit(float R, float G, float B, doubl
   const double ty = fma(kk.mw[1][2], b, fma(kk.mw[1][1], g, kk.mw[1][0] * r));
   const double tz = fma(kk.mw[2][2], b, fma(kk.mw[2][1], g, kk.mw[2][0] * r));
   double x, y, z;
-  if (min(__double2hiint(tx), min(__double2hiint(ty), __double2hiint(tz))) > kCieEpsHi) {
+  // every ratio in (216/24389, 2): each high word above the epsilon's (signed: a negative ratio's word is below it), and the
+  // top exponent bit -- set for 2 and above, +inf and NaN -- clear in all three
+  const int hx = __double2hiint(tx), hy = __double2hiint(ty), hz = __double2hiint(tz);
+  if (min(hx, min(hy, hz)) > kCieEpsHi && ((hx | hy | hz) & kTwoAndAboveBit) == 0) {
     x = cube_root5(tx); y = cube_root5(ty); z = cube_root5(tz);
   } else { x = lab_f_toe(tx); y = lab_f_toe(ty); z = lab_f_toe(tz); }
   o0 = __dsub_rn(__dmul_rn(kk.c116, y), kk.c16) * kk.l_scale;     // unfused: 116*(16/116) - 16 must be exactly 0 (black)
@@ -147,7 +158,7 @@ __global__ void __launch_bounds__(256) colorspace_kernel(float *buf, size_t npix
   if (MODE == kToLinear) {
     o0 = decode_pixel_gamma_tab(in0, s_scale); o1 = decode_pixel_gamma_tab(in1, s_scale); o2 = decode_pixel_gamma_tab(in2, s_scale);
   } else if (MODE == kFromLinear) {
-    o0 = encode_pixel_gamma(in0); o1 = encode_pixel_gamma(in1); o2 = encode_pixel_gamma(in2);
+    o0 = encode_pixel_gamma<true>(in0); o1 = encode_pixel_gamma<true>(in1); o2 = encode_pixel_gamma<true>(in2);
   } else if (MODE == kToLab) {
     rgb_to_lab_unit(in0, in1, in2, o0, o1, o2, s_scale);
   } else if (MODE == kToXyz) {
@@ -168,7 +179,7 @@ __global__ void __launch_bounds__(256) colorspace_kernel(float *buf, size_t npix
       if ((z * z * z) > kCieEps) z = (z * z * z); else z = __dsub_rn(__dmul_rn(116.0, z), 16.0) * (1.0 / kCieK);
       X = kIllX * x; Y = kIllY * y; Z = kIllZ * z;
     }
-    xyz_to_rgb(X, Y, Z, o0, o1, o2);
+    xyz_to_rgb<true>(X, Y, Z, o0, o1, o2);
   }
   if (CH == 4) *reinterpret_cast<float4 *>(q) = make_float4(static_cast<float>(o0), static_cast<float>(o1), static_cast<float>(o2), in3);
   else { q[0] = static_cast<float>(o0); q[1] = static_cast<float>(o1); q[2] = static_cast<float>(o2); }
@@ -311,7 +322,7 @@ __global__ void __launch_bounds__(256) xyz_family_kernel(float *buf, size_t npix
       o0 = QR * J; o1 = QR * a; o2 = QR * b;
     } else {
       jzazbz_to_xyz(st.white_luminance, QS * static_cast<double>(in0), QS * static_cast<double>(in1), QS * static_cast<double>(in2), X, Y, Z);
-      xyz_to_rgb(X, Y, Z, o0, o2, o1);
+      xyz_to_rgb<true>(X, Y, Z, o0, o2, o1);
     }
   } else if (space == MB200_OklabColorspace || space == MB200_OklchColorspace) {      // colorspace-private.h:1480-1549
     if (forward) {
@@ -339,9 +350,9 @@ __global__ void __launch_bounds__(256) xyz_family_kernel(float *buf, size_t npix
       double m = L - 0.1055613458 * (a - 0.5) - 0.0638541728 * (b - 0.5);
       double t = L - 0.0894841775 * (a - 0.5) - 1.2914855480 * (b - 0.5);
       l *= l * l; m *= m * m; t *= t * t;
-      o0 = encode_pixel_gamma(QR * (4.0767416621 * l - 3.3077115913 * m + 0.2309699292 * t));
-      o1 = encode_pixel_gamma(QR * (-1.2684380046 * l + 2.6097574011 * m - 0.3413193965 * t));
-      o2 = encode_pixel_gamma(QR * (-0.0041960863 * l - 0.7034186147 * m + 1.7076147010 * t));
+      o0 = encode_pixel_gamma<true>(QR * (4.0767416621 * l - 3.3077115913 * m + 0.2309699292 * t));
+      o1 = encode_pixel_gamma<true>(QR * (-1.2684380046 * l + 2.6097574011 * m - 0.3413193965 * t));
+      o2 = encode_pixel_gamma<true>(QR * (-0.0041960863 * l - 0.7034186147 * m + 1.7076147010 * t));
     }
   } else if (forward) {
     double X, Y, Z, a, b, c;
@@ -363,7 +374,7 @@ __global__ void __launch_bounds__(256) xyz_family_kernel(float *buf, size_t npix
       xyz_to_lab_unit(st, X, Y, Z, a, b, c);
     } else if (rgb >= 0) {
       mul3(kx.to_rgb[rgb], X, Y, Z, a, b, c);
-      a = QS * encode_pixel_gamma(QR * a); b = QS * encode_pixel_gamma(QR * b); c = QS * encode_pixel_gamma(QR * c);
+      a = QS * encode_pixel_gamma<true>(QR * a); b = QS * encode_pixel_gamma<true>(QR * b); c = QS * encode_pixel_gamma<true>(QR * c);
     } else if (space == MB200_LMSColorspace) {
       mul3(kx.xyz_to_lms, X, Y, Z, a, b, c);
     } else if (space == MB200_CAT02LMSColorspace) {
@@ -403,7 +414,7 @@ __global__ void __launch_bounds__(256) xyz_family_kernel(float *buf, size_t npix
     } else {                                                       // Luv
       luv_to_xyz_d(st, 100.0 * a, 354.0 * b - 134.0, 262.0 * c - 140.0, X, Y, Z);
     }
-    xyz_to_rgb(X, Y, Z, o0, o1, o2);
+    xyz_to_rgb<true>(X, Y, Z, o0, o1, o2);
   }
   if (CH == 4) *reinterpret_cast<float4 *>(q) = make_float4(static_cast<float>(o0), static_cast<float>(o1), static_cast<float>(o2), in3);
   else { q[0] = static_cast<float>(o0); q[1] = static_cast<float>(o1); q[2] = static_cast<float>(o2); }

@@ -123,11 +123,11 @@ __device__ __forceinline__ double encode_pixel_gamma(double pixel) {   // pixel.
 constexpr double kIllX = 0.95047, kIllY = 1.00000, kIllZ = 1.08883;   // D65
 constexpr double kCieEps = 216.0 / 24389.0, kCieK = 24389.0 / 27.0;
 
-// t^(1/3) for t in (216/24389, ~1.3]: z0 = 2^(-log2(t)/3) in fp32 (MUFU, ~2^-21), then one Newton step on
-// z = t^(-1/3) folded into the result: t*z1^2 with z1 = z0*(1 + e/3) is w*(1 + 2e/3) + O(e^2), w = t*z0^2, e = 1 - w*z0
-// (|e| < 2^-20, so the dropped e^2/9 term is below 2^-43) -- five FP64 operations.
-// (lg2 / ex2 as the bare MUFU instructions: t is in (0.0088, ~1.4], so neither needs the range handling of log2f / exp2f,
-// which costs two divergent-branch regions per call.)
+// t^(1/3) for t in (216/24389, 2) (~1.3 for in-range samples): z0 = 2^(-log2(t)/3) in fp32 (MUFU, ~2^-21), then one
+// Newton step on z = t^(-1/3) folded into the result: t*z1^2 with z1 = z0*(1 + e/3) is w*(1 + 2e/3) + O(e^2), w = t*z0^2,
+// e = 1 - w*z0 (|e| < 2^-20, so the dropped e^2/9 term is below 2^-43) -- five FP64 operations.
+// (lg2 / ex2 as the bare MUFU instructions: t is in (0.0088, 2), so neither needs the range handling of log2f / exp2f,
+// which costs two divergent-branch regions per call.  Other t: cube_root below.)
 __device__ __forceinline__ double cube_root5(double t) {
   const float tf = static_cast<float>(t);
   float l, zf;
@@ -138,6 +138,14 @@ __device__ __forceinline__ double cube_root5(double t) {
   const double e = fma(-w, z0, 1.0);
   return fma(w * e, kk.two_thirds, w);
 }
+
+// pow(t, 1/3) for every t above the CIE epsilon: cube_root5 below 2, the range of every sample up to ~1.35 QuantumRange;
+// above, cbrt (1 double ULP), which differs from the reference's pow(t, 0.333...) by a relative 1.9e-17 * ln(t) < 1.4e-14.
+// (The seed's error grows with |log2 t|: one Newton step leaves ~3e-11 relative at t = 2^73 and, from t ~ 2^128 -- HDRI
+// samples from ~7e20 up -- (float) t overflows and the seed is 0.  Lab's a / b of a near-gray pixel is a difference of
+// two cube roots, which brings such an error up to float precision.)
+constexpr double kCubeRootSeedMax = 2.0;
+__device__ __forceinline__ double cube_root(double t) { return t < kCubeRootSeedMax ? cube_root5(t) : cbrt(t); }
 
 template <bool NONFINITE = false>
 __device__ __forceinline__ void xyz_to_rgb(double X, double Y, double Z, double &R, double &G, double &B) {
@@ -166,7 +174,7 @@ struct XyzSettings {
 };
 
 // Lab in unit range (colorspace-private.h:1066-1089) and back (:531-557), for the polar LCHab space
-__device__ __forceinline__ double lab_f(double t) { return t > kCieEps ? cube_root5(t) : (kCieK * t + 16.0) / 116.0; }
+__device__ __forceinline__ double lab_f(double t) { return t > kCieEps ? cube_root(t) : (kCieK * t + 16.0) / 116.0; }
 __device__ __forceinline__ void xyz_to_lab_unit(const XyzSettings &st, double X, double Y, double Z, double &L, double &a, double &b) {
   const double x = lab_f(X / st.ill[0]), y = lab_f(Y / st.ill[1]), z = lab_f(Z / st.ill[2]);
   L = __dsub_rn(__dmul_rn(116.0, y), 16.0) / 100.0;
@@ -182,7 +190,7 @@ __device__ __forceinline__ void lab_to_xyz_d(const XyzSettings &st, double L, do
   X = st.ill[0] * x; Y = st.ill[1] * y; Z = st.ill[2] * z;
 }
 __device__ __forceinline__ void xyz_to_luv_unit(const XyzSettings &st, double X, double Y, double Z, double &L, double &u, double &v) {
-  double l = Y > kCieEps ? __dsub_rn(__dmul_rn(116.0, cube_root5(Y)), 16.0) : kCieK * Y;
+  double l = Y > kCieEps ? __dsub_rn(__dmul_rn(116.0, cube_root(Y)), 16.0) : kCieK * Y;
   const double alpha = perceptible_reciprocal_d(X + 15.0 * Y + 3.0 * Z);
   const double uu = 13.0 * l * (4.0 * alpha * X - st.un), vv = 13.0 * l * (9.0 * alpha * Y - st.vn);
   L = l / 100.0; u = (uu + 134.0) / 354.0; v = (vv + 140.0) / 262.0;

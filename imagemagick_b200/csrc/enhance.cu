@@ -67,7 +67,7 @@ __global__ void __launch_bounds__(256) contrast_kernel(float *buf, size_t npixel
   load_px<CH, VEC>(q, v);
   double r, g, b;
   get_rgb<CH>(v, r, g, b);
-  const Triple t = to_hsb<true>(r, g, b);                                                                      // enhance.c:1381
+  const Triple t = to_hsb(r, g, b);                                                                      // enhance.c:1381
   // brightness += 0.5*sign*(0.5*(sin(MagickPI*(brightness-0.5))+1.0)-brightness)
   double brightness = ad(t.z, ml(half_sign, sb(ml(0.5, ad(sin(ml(kMagickPI, sb(t.z, 0.5))), 1.0)), t.z)));
   if (brightness > 1.0) brightness = 1.0;
@@ -138,7 +138,7 @@ __global__ void __launch_bounds__(256) modulate_kernel(float *buf, size_t npixel
       o = a.space == kModHCL ? from_hcl<false>(t.x, t.y, t.z) : from_hcl<true>(t.x, t.y, t.z);
       break;
     case kModHSB:
-      t = to_hsb<true>(r, g, b);
+      t = to_hsb(r, g, b);
       t.x = ad(t.x, a.hue_shift); t.y = ml(t.y, a.saturation); t.z = ml(t.z, a.brightness);
       o = from_hsb(t.x, t.y, t.z);
       break;

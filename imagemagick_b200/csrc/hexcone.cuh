@@ -63,13 +63,11 @@ __device__ Triple to_hcl(double r, double g, double b) {                        
 }
 
 // ConvertRGBToHSB takes its extremes as max(max(red, green), blue), the other legs as max(red, max(green, blue)); the two
-// differ only where a sample is NaN.  REF_NAN keeps the reference's order (Contrast and Modulate); the colourspace
-// transform (hexcone.cu) still takes the other one.
-template <bool REF_NAN = false>
+// differ only where a sample is NaN, so the order is kept.
 __device__ Triple to_hsb(double r, double g, double b) {                        // :867
-  const double top = REF_NAN ? hi3(b, r, g) : hi3(r, g, b);
+  const double top = hi3(b, r, g);
   if (tiny(top)) return {0.0, 0.0, 0.0};
-  const double span = sb(top, REF_NAN ? lo3(b, r, g) : lo3(r, g, b));
+  const double span = sb(top, lo3(b, r, g));
   Triple t{0.0, dv(span, top), ml(QS, top)};
   if (tiny(span)) return t;
   double h;

@@ -180,7 +180,6 @@ def test_hop_out_of_layout(space, layout):
     function of its input (the polar hue of LCHab and the tabled Log / YCC legs take the composition check only)."""
     for alpha in (False, True):
         src = lc.source(layout, alpha, w=23, seed=space)
-        src = np.nan_to_num(src, nan=100.0, posinf=70000.0, neginf=-5.0)
         for got in gpu_both(src, layout, space):
             rc, rgb, _ = run_dev(src, layout, lc.SRGB)
             assert rc == 0
