@@ -62,6 +62,9 @@ __device__ __forceinline__ double pixel_intensity(const float (&v)[CH]) {
 }
 
 // ------------------------------------------------------------------------------------------------ StatisticImage
+// MagickAbsoluteValue (image-private.h:45): unlike fabs it keeps -0 (Contrast of a one-level window of negative samples)
+__device__ __forceinline__ double magick_absolute_value(double x) { return x < 0.0 ? -x : x; }
+
 __device__ __forceinline__ unsigned scale_quantum_to_short(float q) {      // quantum-private.h (HDRI)
   if (!(q > 0.0f)) return 0u;
   if (q >= 65535.0f) return 65535u;
@@ -215,7 +218,7 @@ __global__ void __launch_bounds__(128) statistic_kernel(const float *__restrict_
   for (int c = 0; c < CH; ++c) {
     double pixel;
     switch (type) {
-      case 1: pixel = fabs(__dsub_rn(maximum[c], minimum[c])); break;
+      case 1: pixel = magick_absolute_value(__dsub_rn(maximum[c], minimum[c])); break;
       case 2: pixel = maximum[c]; break;
       case 5: pixel = minimum[c]; break;
       case 8: pixel = __dsqrt_rn(__ddiv_rn(sum_squared[c], area)); break;
@@ -224,7 +227,7 @@ __global__ void __launch_bounds__(128) statistic_kernel(const float *__restrict_
         pixel = __dsqrt_rn(__dsub_rn(__ddiv_rn(sum_squared[c], area), m));
         break;
       }
-      case 10: pixel = fabs(__dmul_rn(__dsub_rn(maximum[c], minimum[c]), perceptible_reciprocal(__dadd_rn(maximum[c], minimum[c])))); break;
+      case 10: pixel = magick_absolute_value(__dmul_rn(__dsub_rn(maximum[c], minimum[c]), perceptible_reciprocal(__dadd_rn(maximum[c], minimum[c])))); break;
       default: pixel = __ddiv_rn(sum[c], area); break;
     }
     o[c] = static_cast<float>(pixel);
@@ -355,8 +358,8 @@ __global__ void __launch_bounds__(128) bilateral_kernel(const float *__restrict_
 
 // -------------------------------------------------------------------------------------------- SelectiveBlurImage
 // Double intensity plane (one pre-pass): the reference compares the centre's double intensity with, for the alpha-blended
-// colour channels, the neighbour's double intensity (:3640) and, for the others, the FLOAT it stored in its GRAY clone
-// (colorspace.c:943) -- which is the same double rounded to float, so one plane serves both.
+// colour channels, the neighbour's double intensity (:3657) and, for the others, the neighbour's intensity in its GRAY
+// clone (:3629), which gray_clone_intensity derives from the same plane.
 template <int CH>
 __global__ void __launch_bounds__(256) intensity_plane_kernel(const float *__restrict__ src, double *__restrict__ out, size_t n) {
   const size_t i = static_cast<size_t>(blockIdx.x) * 256 + threadIdx.x;
@@ -364,6 +367,17 @@ __global__ void __launch_bounds__(256) intensity_plane_kernel(const float *__res
   float v[CH];
   load_pixel<CH>(src, i, v);
   out[i] = pixel_intensity<CH>(v);
+}
+
+// GetPixelIntensity of the GRAY clone's pixel, from the pixel's double intensity li.  The clone stores li rounded to
+// float (colorspace.c:943-945); a gray image is not transformed, and its li is already its sample.  With alpha the clone
+// keeps two channels, so the intensity weighs its sample as (g, g, g) again (pixel.c:2366) -- for a gray image that is
+// li itself.
+template <int CH>
+__device__ __forceinline__ double gray_clone_intensity(double li) {
+  if (CH == 2) return li;
+  const float g[2] = {static_cast<float>(li), 0.0f};
+  return CH == 4 ? pixel_intensity<2>(g) : static_cast<double>(g[0]);
 }
 
 // window top-left (x - j, y - j), j = (width-1)/2, edge replicated; taps in window order, unfused.
@@ -386,7 +400,7 @@ __global__ void __launch_bounds__(128) selective_blur_kernel(const float *__rest
     for (int u = 0; u < W; ++u, ++k) {
       const size_t idx = row + min(max(x - j + u, 0), w - 1);
       const double li = __ldg(lum + idx);
-      const bool take_plain = fabs(__dsub_rn(static_cast<double>(static_cast<float>(li)), intensity)) < threshold;
+      const bool take_plain = fabs(__dsub_rn(gray_clone_intensity<CH>(li), intensity)) < threshold;
       const bool take_blend = kAlpha && fabs(__dsub_rn(li, intensity)) < threshold;
       if (!take_plain && !take_blend) continue;
       const double t = __ldg(taps + k);
@@ -460,37 +474,6 @@ __global__ void __launch_bounds__(128) exact_convolve_kernel(const float *__rest
 #pragma unroll
   for (int c = 0; c < CH; ++c) o[c] = static_cast<float>(__dmul_rn((kAlpha && c != CH - 1) ? g : 1.0, pixel[c]));
   store_pixel<CH>(dst, static_cast<size_t>(y) * w + x, o);
-}
-
-// GetImageRange (statistic.c:1851) over every channel: floats mapped to unsigned keys of the same order (NaN never
-// wins a reference comparison and is skipped), block reduction, one atomicMin / atomicMax per CTA.
-__device__ __forceinline__ unsigned order_key(float f) {
-  const unsigned b = __float_as_uint(f);
-  return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
-}
-__device__ __forceinline__ float key_value(unsigned k) {
-  return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
-}
-__global__ void __launch_bounds__(256) range_kernel(const float *__restrict__ buf, size_t n, unsigned *__restrict__ range) {
-  unsigned lo = 0xffffffffu, hi = 0u;
-  for (size_t i = static_cast<size_t>(blockIdx.x) * 256 + threadIdx.x; i < n; i += static_cast<size_t>(gridDim.x) * 256) {
-    const float f = __ldg(buf + i);
-    if (f == f) { const unsigned k = order_key(f); lo = min(lo, k); hi = max(hi, k); }
-  }
-  lo = __reduce_min_sync(0xffffffffu, lo);
-  hi = __reduce_max_sync(0xffffffffu, hi);
-  if ((threadIdx.x & 31) == 0) { atomicMin(range, lo); atomicMax(range + 1, hi); }
-}
-// LevelImage(min, max, 1.0) + ClampImage (enhance.c:2900-3020, threshold.c:1087) unless |min - max| < MagickEpsilon
-// (histogram.c:950); the decision and PerceptibleReciprocal(max - min) are evaluated on the device from range[].
-__global__ void __launch_bounds__(256) level_clamp_kernel(float *__restrict__ buf, size_t n, const unsigned *__restrict__ range) {
-  const size_t i = static_cast<size_t>(blockIdx.x) * 256 + threadIdx.x;
-  if (i >= n) return;
-  const double minima = static_cast<double>(key_value(range[0])), maxima = static_cast<double>(key_value(range[1]));
-  if (!(fabs(__dsub_rn(minima, maxima)) >= kEps)) return;
-  const double scale = perceptible_reciprocal(__dsub_rn(maxima, minima));
-  const float q = static_cast<float>(__dmul_rn(65535.0, __dmul_rn(scale, __dsub_rn(static_cast<double>(buf[i]), minima))));
-  buf[i] = q < 0.0f ? 0.0f : (q >= 65535.0f ? 65535.0f : q);
 }
 
 // The adaptive stage (effect.c:279-372): j from the edge map's intensity, then the (width - j)^2 window in plain order.
@@ -741,17 +724,10 @@ int exact_convolve(const float *src, float *dst, size_t w, size_t h, int channel
   return e == cudaSuccess ? MB200_OK : cuda_fail(e, "adaptive: convolution launch");
 }
 
-// AutoLevelImage with the default channel mask (enhance.c:266 -> histogram.c:942-953)
-int auto_level(float *buf, size_t n, unsigned *d_range, cudaStream_t s) {
-  static const unsigned init[2] = {0xffffffffu, 0u};
-  cudaError_t e = cudaMemcpyAsync(d_range, init, sizeof(init), cudaMemcpyHostToDevice, s);
-  if (e != cudaSuccess) return cuda_fail(e, "adaptive: range reset");
-  const unsigned blocks = static_cast<unsigned>(std::min<size_t>((n + 255) / 256, static_cast<size_t>(sm_count()) * 16));
-  range_kernel<<<blocks, 256, 0, s>>>(buf, n, d_range);
-  level_clamp_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, s>>>(buf, n, d_range);
-  count_launch(2);
-  e = cudaGetLastError();
-  return e == cudaSuccess ? MB200_OK : cuda_fail(e, "adaptive: auto-level launch");
+// AutoLevelImage with the default channel mask (enhance.c:266 -> histogram.c:942-953): level.cu's MinMaxStretchImage,
+// whose GetImageRange drops a row that starts with NaN as the reference does
+int auto_level(float *buf, size_t w, size_t h, int channels, cudaStream_t s) {
+  return launch_minmax_stretch(buf, w, h, channels, 0.0, 0.0, 1.0, false, (1u << channels) - 1u, s);
 }
 
 struct DeviceTemp {
@@ -804,18 +780,17 @@ int launch_adaptive(const float *src, float *dst, size_t w, size_t h, int channe
   const KernelList edge_k(mb200_edge_kernel(radius)), blur_k = blur_kernel_pair(radius, sigma);
   if (!edge_k || !blur_k) return fail(MB200_ENOMEM, "adaptive: kernels");
 
-  DeviceTemp edge(s), tmp(s), range(s), d_offsets(s);
-  if ((rc = edge.alloc(n * sizeof(float))) || (rc = tmp.alloc(n * sizeof(float))) || (rc = range.alloc(2 * sizeof(unsigned))) ||
+  DeviceTemp edge(s), tmp(s), d_offsets(s);
+  if ((rc = edge.alloc(n * sizeof(float))) || (rc = tmp.alloc(n * sizeof(float))) ||
       (rc = d_offsets.alloc(offsets.size() * sizeof(int))))
     return rc;
   float *d_edge = static_cast<float *>(edge.p), *d_tmp = static_cast<float *>(tmp.p);
-  unsigned *d_range = static_cast<unsigned *>(range.p);
   // EdgeImage -> AutoLevel -> BlurImage (row kernel, then the rotated one: float intermediate) -> AutoLevel
   if ((rc = exact_convolve(src, d_edge, w, h, channels, edge_k.get(), s))) return rc;
-  if ((rc = auto_level(d_edge, n, d_range, s))) return rc;
+  if ((rc = auto_level(d_edge, w, h, channels, s))) return rc;
   if ((rc = exact_convolve(d_edge, d_tmp, w, h, channels, blur_k.get(), s))) return rc;
   if ((rc = exact_convolve(d_tmp, d_edge, w, h, channels, blur_k->next, s))) return rc;
-  if ((rc = auto_level(d_edge, n, d_range, s))) return rc;
+  if ((rc = auto_level(d_edge, w, h, channels, s))) return rc;
 
   double *d_kernels = nullptr;
   if ((rc = upload_table(kernels, &d_kernels, s))) return rc;

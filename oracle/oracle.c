@@ -2628,9 +2628,11 @@ int orc_bilateral_blur(const float *src, float *dst, size_t w, size_t h, int ch,
 /* ------------------------------------------------------------------------------------------
    effect.c:3406-3700 SelectiveBlurImage: a width x width Gaussian (GetOptimalKernelWidth1D, not normalised) of which only
    the taps whose intensity differs from the centre pixel's by less than `threshold` take part.  Channels without the
-   Blend trait (no alpha, or the alpha channel) compare the FLOAT-rounded luminance of the neighbour -- the reference reads
-   it from a clone transformed to GRAYColorspace (colorspace.c:943-945) -- with the centre's double intensity; the
-   alpha-blended colour channels compare double intensities (:3640).  gamma == 0 (no tap qualifies) copies the centre.
+   Blend trait (no alpha, or the alpha channel) compare the neighbour's intensity in a clone transformed to GRAYColorspace
+   (:3629) with the centre's double intensity: the clone holds the FLOAT-rounded intensity (colorspace.c:943-945; a gray
+   image is left as it is), and with alpha it has two channels, so GetPixelIntensity (pixel.c:2366) returns
+   0.212656 g + 0.715158 g + 0.072186 g of that sample rather than g.  The alpha-blended colour channels compare double
+   intensities (:3657).  gamma == 0 (no tap qualifies) copies the centre.
    ------------------------------------------------------------------------------------------ */
 int orc_selective_blur(const float *src, float *dst, size_t w, size_t h, int ch, double radius, double sigma, double threshold)
 {
@@ -2665,7 +2667,11 @@ int orc_selective_blur(const float *src, float *dst, size_t w, size_t h, int ch,
             yy = yy < 0 ? 0 : (yy >= (long) h ? (long) h - 1 : yy);
             r = src + ((size_t) yy * w + (size_t) xx) * ch;
             if (!blend) {
-              contrast = (double) (float) pixel_intensity(r, ch) - intensity;
+              /* the GRAY clone's sample is the float intensity (a gray image's own sample); with alpha the clone
+                 keeps two channels, so GetPixelIntensity weighs that sample as (g, g, g) again */
+              const float g = ch >= 3 ? (float) pixel_intensity(r, ch) : r[0];
+              const double luminance = has_alpha ? 0.212656 * g + 0.715158 * g + 0.072186 * g : (double) g;
+              contrast = luminance - intensity;
               if (fabs(contrast) < threshold) { pixel += (*k) * (double) r[c]; gamma += (*k); }
             } else {
               contrast = pixel_intensity(r, ch) - intensity;
@@ -2805,7 +2811,8 @@ int orc_statistic(const float *src, float *dst, size_t w, size_t h, int ch, int 
             sum_squared += value * value;
           }
         switch (type) {
-          case 1: pixel = fabs(maximum - minimum); break;                                          /* Gradient */
+          /* MagickAbsoluteValue (image-private.h:45), x < 0 ? -x : x, keeps the sign of a zero (and of a NaN) */
+          case 1: pixel = maximum - minimum; pixel = pixel < 0 ? -pixel : pixel; break;              /* Gradient */
           case 2: pixel = maximum; break;
           case 4:
             qsort(list, (size_t) n, sizeof(unsigned short), cmp_ushort);
@@ -2839,7 +2846,10 @@ int orc_statistic(const float *src, float *dst, size_t w, size_t h, int ch, int 
           }
           case 8: pixel = sqrt(sum_squared / area); break;
           case 9: pixel = sqrt(sum_squared / area - (sum / area * sum / area)); break;
-          case 10: pixel = fabs((maximum - minimum) * perceptible_reciprocal(maximum + minimum)); break;
+          case 10:
+            pixel = (maximum - minimum) * perceptible_reciprocal(maximum + minimum);
+            pixel = pixel < 0 ? -pixel : pixel;
+            break;
           default: pixel = sum / area; break;                                                      /* Mean */
         }
         dst[((size_t) y * w + (size_t) x) * ch + c] = (float) pixel;
@@ -2854,8 +2864,8 @@ int orc_statistic(const float *src, float *dst, size_t w, size_t h, int ch, int 
    effect.c:128-416 AdaptiveBlurImage / :447-735 AdaptiveSharpenImage (sharpen != 0).
      edge  = EdgeImage(image, radius)                              (:181)
      AutoLevelImage(edge) = MinMaxStretchImage(edge, 0, 0, 1.0)    (enhance.c:266, histogram.c:927): the default channel
-             mask is AllChannels, so ONE range over every channel (GetImageRange statistic.c:1851: plain comparisons, NaN never
-             wins), LevelImage (enhance.c:2913: QuantumRange * (PerceptibleReciprocal(max - min) * (pixel - min)), gamma 1 so
+             mask is AllChannels, so ONE range over every channel (GetImageRange statistic.c:1851: plain comparisons seeded
+             with each row's first sample, so NaN never wins but a row starting with NaN is dropped), LevelImage (enhance.c:2913: QuantumRange * (PerceptibleReciprocal(max - min) * (pixel - min)), gamma 1 so
              gamma_pow is the identity; skipped when |min - max| < MagickEpsilon) and ClampImage (threshold.c:1087)
      edge  = BlurImage(edge, radius, sigma); AutoLevelImage(edge)  (:188-194)
      width = GetOptimalKernelWidth2D(radius, sigma); kernel[j], j = 0, 2, ..: (width - j)^2 Gaussians, the centre absorbs
@@ -2865,12 +2875,19 @@ int orc_statistic(const float *src, float *dst, size_t w, size_t h, int ch, int 
    ------------------------------------------------------------------------------------------ */
 static void auto_level(float *buf, size_t w, size_t h, int ch)
 {
-  const size_t n = w * h * (size_t) ch;
-  double minima = 1.7976931348623157e308, maxima = -1.7976931348623157e308, scale;   /* MagickMaximumValue / Minimum */
-  size_t i;
-  for (i = 0; i < n; i++) {
-    if ((double) buf[i] < minima) minima = (double) buf[i];
-    if ((double) buf[i] > maxima) maxima = (double) buf[i];
+  const size_t n = w * h * (size_t) ch, row = w * (size_t) ch;
+  double minima = 1.7976931348623157e308, maxima = 2.2250738585072014e-308, scale;   /* MagickMaximumValue / Minimum */
+  size_t i, y;
+  /* GetImageRange seeds each row's extremes with the row's first sample, so a row that starts with NaN stays NaN and
+     the merge drops it whole (statistic.c:1895-1896, :1921-1924) */
+  for (y = 0; y < h; y++) {
+    double row_minima = (double) buf[y * row], row_maxima = row_minima;
+    for (i = y * row; i < (y + 1) * row; i++) {
+      if ((double) buf[i] < row_minima) row_minima = (double) buf[i];
+      if ((double) buf[i] > row_maxima) row_maxima = (double) buf[i];
+    }
+    if (row_minima < minima) minima = row_minima;
+    if (row_maxima > maxima) maxima = row_maxima;
   }
   if (!(fabs(minima - maxima) >= EPS)) return;
   scale = perceptible_reciprocal(maxima - minima);
