@@ -1,5 +1,5 @@
 // conv_mma.cu -- one pass of a separable (1-D) convolution on RGBA images, evaluated on the FP64 matrix path
-// (mma.sync.m8n8k4.f64, SASS DMMA).  Same semantics as conv1d.cu (MorphologyPrimitive's ConvolveMorphology for
+// (mma.sync.m8n8k4.f64, SASS DMMA.8x8x4; windows of 18-33 taps on mma.sync.m16n8k16.f64, see conv_mma_wide_kernel).  Same semantics as conv1d.cu (MorphologyPrimitive's ConvolveMorphology for
 // height-1 / width-1 kernels, MagickCore/morphology.c:2897-2979 and :2654-2807: reflected taps, edge-clamped source,
 // double accumulation, alpha-weighted colour channels, one rounding to float).
 //
@@ -47,7 +47,7 @@ struct MmaArgs {
   int width, height;      // pixels
   int off;                // samples of the window before the output position
   int ntaps;
-  int strip;              // outputs per strip along the filter axis (multiple of 8)
+  int strip;              // outputs per strip along the filter axis (multiple of 8; of 16 for the wide tiles)
   const float *aux;       // EPI = 1: UnsharpMaskImage's source image
   double gain, qthreshold;
   int l2pf;               // prefetch.global.L2 ahead of the register prefetch
@@ -351,6 +351,335 @@ __global__ void __launch_bounds__(128, MINB) conv_mma_kernel(const MmaArgs a, co
   output(prev, epi_prev, prev_valid);
 }
 
+// ---- the wide-tile pass: mma.sync.m16n8k16.f64 (SASS DMMA.16x8x16), RGBA float in / float out.
+//
+//   D[m][n] += A_s[m][k] * B_s[k][n]    m = 16 consecutive outputs, k = 16 consecutive source samples (k-step s of NKS),
+//                                       n = 8 component lines;  A_s[m][k] = tap[16 s + k - m]
+//
+// One DMMA.16x8x16 carries 2048 FMAs: 4 tiles x NKS = 12 DMMAs per 16 outputs x 8 pixel lines of a 33-tap window, where
+// conv_mma_kernel issues 80 DMMA.8x8x4 (tools/micro/dmma.cu and dmma_feed.cu measure both shapes).  Fragment
+// coordinates (g = lane / 4, t = lane % 4): A element i at (m = g + 8 (i & 1), k = t + 4 (i >> 1)), B element i at
+// (k = t + 4 i, n = g), D element i at (m = g + 8 (i >> 1), n = 2 t + (i & 1)).  The n mapping is conv_mma_kernel's, so a
+// lane ends up with all four sums of pixel line 4 G + t (tile group G) at outputs g and g + 8.
+//
+// Everything else is conv_mma_kernel's scheme at 16-position blocks: a per-warp ring of NKS + 1 blocks (the window and
+// the block being refilled), samples converted and premultiplied once when staged, one non-finite flag per block, loads
+// two blocks ahead of the ring, and the DMMAs of block b, the staging of block b + NKS and the output stage of block
+// b - 1 in one basic block.  Outputs start at multiples of 16 of the image position (the launcher rounds the strip up),
+// so an output's k-grouping, and its bits, do not depend on the strip.
+template <int NKS>
+struct WideTaps { double k[16 * NKS]; };    // window order, zero past the window
+
+template <int NKS, int AXIS, int EPI>
+__global__ void __launch_bounds__(128, 3) conv_mma_wide_kernel(const MmaArgs a, const WideTaps<NKS> taps) {
+  static_assert(EPI == 0 || AXIS == 1, "the fused epilogue belongs to the final column pass");
+  constexpr int NB = NKS + 1;                      // ring blocks: the window + the one being refilled
+  constexpr int RR = 16 * NB;                      // ring positions along the filter axis
+  constexpr int PW = 36;                           // AXIS 1: doubles per ring row: [RG of 8 px | BA of 8 px | pad 4]
+  constexpr int PL = 2 * RR + 8;                   // AXIS 0: doubles per image line of a plane (== 8 mod 16)
+  constexpr int kWarpDoubles = AXIS == 1 ? RR * PW : 16 * PL;
+  extern __shared__ __align__(16) double ring_all[];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  double *ring = ring_all + warp * kWarpDoubles;
+  const unsigned ring_s = static_cast<unsigned>(__cvta_generic_to_shared(ring));
+  const int t4 = lane & 3, g8 = lane >> 2;
+
+  int first, nout, limit, par0;
+  if (AXIS == 1) {
+    par0 = (blockIdx.x * 4 + warp) * 8;
+    if (par0 >= a.width) return;                   // (no CTA-wide barrier anywhere: a warp may leave)
+    first = blockIdx.y * a.strip;
+    nout = min(a.strip, a.height - first);
+    limit = a.height - 1;
+  } else {
+    par0 = (blockIdx.y * 4 + warp) * 8;
+    if (par0 >= a.height) return;
+    first = blockIdx.x * a.strip;
+    nout = min(a.strip, a.width - first);
+    limit = a.width - 1;
+  }
+  const int nblocks = (nout + 15) >> 4;
+  const bool mma_l2pf = a.l2pf != 0;
+  const size_t pitch = static_cast<size_t>(a.width) * 16;
+
+  // ---- loader: four pixels per lane and block
+  const int lq = lane & 7, lh = lane >> 3;
+  const char *lbase[4];
+  int uoff[4];
+  unsigned st_off[4];                              // ring offset (doubles) of the RG pair inside block slot 0
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    if (AXIS == 1) {                               // rows lh + 4 i of the block, pixel column lq
+      lbase[i] = static_cast<const char *>(a.src) + static_cast<size_t>(min(par0 + lq, a.width - 1)) * 16;
+      uoff[i] = lh + 4 * i;
+      st_off[i] = static_cast<unsigned>(uoff[i] * PW + 2 * lq);
+    } else {                                       // image line lh + 4 (i >> 1), positions lq + 8 (i & 1) of the block
+      const int line = lh + 4 * (i >> 1);
+      lbase[i] = static_cast<const char *>(a.src) + static_cast<size_t>(min(par0 + line, a.height - 1)) * pitch;
+      uoff[i] = lq + 8 * (i & 1);
+      st_off[i] = static_cast<unsigned>(line * PL + 2 * uoff[i]);
+    }
+  }
+  constexpr unsigned kBlockStride = AXIS == 1 ? 16 * PW : 32;     // ring doubles per block slot
+  constexpr unsigned kBA = AXIS == 1 ? 16 : 8 * PL;               // RG -> BA plane
+  const size_t lstep = AXIS == 1 ? pitch : 16;
+  const int base = first - a.off;                  // source position of ring block 0, element 0
+
+  float4 raw[4];
+  auto fetch = [&](int j) {
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const unsigned pos = static_cast<unsigned>(min(max(base + 16 * j + uoff[i], 0), limit));
+      raw[i] = __ldg(reinterpret_cast<const float4 *>(lbase[i] + static_cast<size_t>(pos) * lstep));
+    }
+  };
+  constexpr int kL2Ahead = 4;
+  auto prefetch_l2 = [&](int j) {
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const unsigned pos = static_cast<unsigned>(min(max(base + 16 * j + uoff[i], 0), limit));
+      asm volatile("prefetch.global.L2 [%0];" ::"l"(lbase[i] + static_cast<size_t>(pos) * lstep));
+    }
+  };
+  unsigned badmask = 0;
+  auto stage = [&](int slot) {                     // registers -> ring block `slot`; updates the block's flag
+    bool bad = false;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const float4 f = raw[i];
+      const unsigned m = max(max(__float_as_uint(f.x) & 0x7fffffffu, __float_as_uint(f.y) & 0x7fffffffu),
+                             max(__float_as_uint(f.z) & 0x7fffffffu, __float_as_uint(f.w) & 0x7fffffffu));
+      bad = bad || m >= 0x7f800000u;
+      const double da = static_cast<double>(f.w);
+      double *q = ring + st_off[i] + static_cast<unsigned>(slot) * kBlockStride;
+      *reinterpret_cast<double2 *>(q) = make_double2(static_cast<double>(f.x) * da, static_cast<double>(f.y) * da);
+      *reinterpret_cast<double2 *>(q + kBA) = make_double2(static_cast<double>(f.z) * da, da);
+    }
+    const bool any = __any_sync(0xffffffffu, bad);
+    badmask = any ? (badmask | (1u << slot)) : (badmask & ~(1u << slot));
+  };
+
+  // ---- tap tiles: element i of A_s is tap[16 s + t4 + 4 (i >> 1) - g8 - 8 (i & 1)] = atap[c + 2] with
+  // c = 4 s + (i >> 1) - 2 (i & 1): 4 NKS + 2 distinct doubles per lane instead of 8 NKS
+  constexpr int NA = 4 * NKS + 2;
+  double atap[NA];
+#pragma unroll
+  for (int c = 0; c < NA; ++c) {
+    const int t = 4 * (c - 2) + t4 - g8;
+    const double v = taps.k[min(max(t, 0), 16 * NKS - 1)];
+    atap[c] = (t >= 0 && t < a.ntaps) ? v : 0.0;
+  }
+
+  // ---- B fragment addressing: element i of k-step s reads ring position 16 (sb + s) + t4 + 4 i, column g8
+  const unsigned frag_off = AXIS == 1 ? static_cast<unsigned>(t4 * PW + g8)
+                                      : static_cast<unsigned>(2 * t4 + (g8 >> 1) * PL + (g8 & 1));
+  constexpr unsigned kUStride = AXIS == 1 ? PW : 2;             // ring doubles per position
+  constexpr unsigned kT2 = AXIS == 1 ? 8 : 4 * PL;              // tile group 1
+  constexpr unsigned kTile[4] = {0, kBA, kT2, kT2 + kBA};       // (G, plane) = (0, RG), (0, BA), (1, RG), (1, BA)
+  const unsigned lane_px_off = AXIS == 1 ? static_cast<unsigned>(2 * t4) : static_cast<unsigned>(t4 * PL);
+
+  // ---- output stage: the lane holds pixel line 4 G + t4 at outputs g8 and g8 + 8 of a block
+  char *outp;                                      // output of (block, m = g8, G = 0); lags the MMAs by one block
+  if (AXIS == 1) {
+    outp = static_cast<char *>(a.dst) + static_cast<size_t>(first + g8) * pitch + static_cast<size_t>(par0 + t4) * 16;
+  } else {
+    outp = static_cast<char *>(a.dst) + static_cast<size_t>(par0 + t4) * pitch + static_cast<size_t>(first + g8) * 16;
+  }
+  const size_t ostep = AXIS == 1 ? 16 * pitch : 16 * 16;          // per block
+  const size_t gstep = AXIS == 1 ? 4 * 16 : 4 * pitch;            // G 0 -> 1
+  const size_t hstep = AXIS == 1 ? 8 * pitch : 8 * 16;            // output g8 -> g8 + 8
+  bool gvalid[2];
+#pragma unroll
+  for (int g = 0; g < 2; ++g) gvalid[g] = (par0 + 4 * g + t4) < (AXIS == 1 ? a.width : a.height);
+  auto output = [&](const double (&acc)[4][4], const float4 (&epi)[2][2], int mrem) {    // mrem: outputs left in the block
+#pragma unroll
+    for (int g = 0; g < 2; ++g)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const double sr = acc[2 * g][2 * h], sg = acc[2 * g][2 * h + 1], sbv = acc[2 * g + 1][2 * h],
+                     sa = acc[2 * g + 1][2 * h + 1];
+        const double r = fast_reciprocal(clamp_denominator(sa));
+        float4 out = make_float4(static_cast<float>(sr * r), static_cast<float>(sg * r), static_cast<float>(sbv * r),
+                                 static_cast<float>(sa));
+        if (EPI) {
+          out.x = unsharp_point(epi[g][h].x, out.x, a.gain, a.qthreshold);
+          out.y = unsharp_point(epi[g][h].y, out.y, a.gain, a.qthreshold);
+          out.z = unsharp_point(epi[g][h].z, out.z, a.gain, a.qthreshold);
+          out.w = unsharp_point(epi[g][h].w, out.w, a.gain, a.qthreshold);
+        }
+        if (g8 + 8 * h < mrem && gvalid[g]) *reinterpret_cast<float4 *>(outp + g * gstep + h * hstep) = out;
+      }
+  };
+
+  // ---- prologue: the NKS blocks of the first window (all loads in flight together), then the two blocks after it
+  {
+    float4 pre[NKS][4];
+#pragma unroll
+    for (int j = 0; j < NKS; ++j) {
+      fetch(j);
+#pragma unroll
+      for (int i = 0; i < 4; ++i) pre[j][i] = raw[i];
+    }
+#pragma unroll
+    for (int j = 0; j < NKS; ++j) {
+#pragma unroll
+      for (int i = 0; i < 4; ++i) raw[i] = pre[j][i];
+      stage(j);
+    }
+  }
+  float4 ahead[4];                                 // the block after the one in `raw`
+  fetch(NKS + 1);
+#pragma unroll
+  for (int i = 0; i < 4; ++i) ahead[i] = raw[i];
+  fetch(NKS);
+
+  int st_slot = NKS, sb = 0;                       // slot staged in this iteration / first slot of the window
+  double prev[4][4];
+#pragma unroll
+  for (int t = 0; t < 4; ++t)
+#pragma unroll
+    for (int i = 0; i < 4; ++i) prev[t][i] = (i & 1) ? 1.0 : 0.0;
+  float4 epi_prev[2][2], epi_cur[2][2];
+#pragma unroll
+  for (int g = 0; g < 2; ++g)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) epi_prev[g][h] = epi_cur[g][h] = make_float4(0.f, 0.f, 0.f, 0.f);
+  int prev_rem = 0;                                // block -1 does not exist
+
+#pragma unroll 1
+  for (int b = 0; b < nblocks; ++b) {
+    __syncwarp();
+    const int mrem = nout - 16 * b;
+    const unsigned window_bad = badmask & ~(1u << st_slot);     // flags of the slots this block's windows read
+    // Output stage of the previous block and staging of the next one come BEFORE this block's DMMAs in the source, so
+    // that `prev` and the staged registers are dead while the accumulators and B fragments are live (168 registers at
+    // three CTAs per SM); ptxas still interleaves them with the DMMAs, which are in the same basic block.
+    output(prev, epi_prev, prev_rem);
+    if (b > 0) outp += ostep;
+    if (EPI) {                                     // the source pixels of block b: aux at outp's offset (outp is at block b here)
+      const char *epip = reinterpret_cast<const char *>(a.aux) + (outp - static_cast<char *>(a.dst));
+#pragma unroll
+      for (int g = 0; g < 2; ++g)
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+          if (g8 + 8 * h < mrem && gvalid[g])
+            epi_cur[g][h] = __ldg(reinterpret_cast<const float4 *>(epip + g * gstep + h * hstep));
+    }
+    // next source block -> ring (the slot no window of this iteration reads; the __syncwarp above orders it after the
+    // previous iteration's reads), the one after it -> registers
+    stage(st_slot);
+#pragma unroll
+    for (int i = 0; i < 4; ++i) raw[i] = ahead[i];
+    {
+      float4 keep[4];
+#pragma unroll
+      for (int i = 0; i < 4; ++i) keep[i] = raw[i];
+      fetch(b + NKS + 2);
+      if (mma_l2pf) prefetch_l2(b + NKS + 2 + kL2Ahead);
+#pragma unroll
+      for (int i = 0; i < 4; ++i) { ahead[i] = raw[i]; raw[i] = keep[i]; }
+    }
+    double acc[4][4];
+#pragma unroll
+    for (int t = 0; t < 4; ++t)
+#pragma unroll
+      for (int i = 0; i < 4; ++i) acc[t][i] = 0.0;
+    {
+      // B fragments, one (k-step, tile) at a time, loaded one DMMA ahead (a DMMA.16x8x16 occupies the pipe for ~64
+      // cycles, longer than an LDS takes)
+      unsigned ua[NKS];
+#pragma unroll
+      for (int s = 0; s < NKS; ++s) {
+        const int blk = sb + s >= NB ? sb + s - NB : sb + s;
+        ua[s] = ring_s + (frag_off + static_cast<unsigned>(blk) * kBlockStride) * 8u;
+      }
+      auto lds4 = [&](double (&bv)[4], int q) {
+        const unsigned addr = ua[q >> 2] + kTile[q & 3] * 8;          // (q is unrolled: the offsets fold into the LDS)
+#pragma unroll
+        for (int i = 0; i < 4; ++i)
+          asm volatile("ld.shared.f64 %0, [%1];" : "=d"(bv[i]) : "r"(addr + 4 * i * kUStride * 8));
+      };
+      double bq[2][4];
+      lds4(bq[0], 0);
+#pragma unroll
+      for (int q = 0; q < 4 * NKS; ++q) {
+        if (q + 1 < 4 * NKS) lds4(bq[(q + 1) & 1], q + 1);
+        const double *av = atap + 4 * (q >> 2);     // element i: av[(i >> 1) + 2 - 2 (i & 1)]
+        double (&d)[4] = acc[q & 3];
+        const double (&bv)[4] = bq[q & 1];
+        asm volatile("mma.sync.aligned.m16n8k16.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7,%8,%9,%10,%11}, "
+                     "{%12,%13,%14,%15}, {%0,%1,%2,%3};"
+                     : "+d"(d[0]), "+d"(d[1]), "+d"(d[2]), "+d"(d[3])
+                     : "d"(av[2]), "d"(av[0]), "d"(av[3]), "d"(av[1]), "d"(av[4]), "d"(av[2]), "d"(av[5]), "d"(av[3]),
+                       "d"(bv[0]), "d"(bv[1]), "d"(bv[2]), "d"(bv[3]));
+      }
+    }
+    if (window_bad != 0) {
+      // a window of this block holds a non-finite sample: the window's own taps only, in scalar FMAs
+#pragma unroll
+      for (int g = 0; g < 2; ++g)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          double s0 = 0.0, s1 = 0.0, s2 = 0.0, s3 = 0.0;
+          int u = 16 * sb + g8 + 8 * h;
+          if (u >= RR) u -= RR;
+          for (int t = 0; t < a.ntaps; ++t) {
+            const double *p = ring + static_cast<unsigned>(u) * kUStride + lane_px_off + g * kT2;
+            const double2 rg = *reinterpret_cast<const double2 *>(p);
+            const double2 ba = *reinterpret_cast<const double2 *>(p + kBA);
+            const double k = taps.k[t];
+            s0 = fma(k, rg.x, s0); s1 = fma(k, rg.y, s1); s2 = fma(k, ba.x, s2); s3 = fma(k, ba.y, s3);
+            if (++u == RR) u = 0;
+          }
+          acc[2 * g][2 * h] = s0; acc[2 * g][2 * h + 1] = s1; acc[2 * g + 1][2 * h] = s2; acc[2 * g + 1][2 * h + 1] = s3;
+        }
+    }
+#pragma unroll
+    for (int t = 0; t < 4; ++t)
+#pragma unroll
+      for (int i = 0; i < 4; ++i) prev[t][i] = acc[t][i];
+    if (EPI) {
+#pragma unroll
+      for (int g = 0; g < 2; ++g)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) epi_prev[g][h] = epi_cur[g][h];
+    }
+    prev_rem = mrem;
+    st_slot = st_slot + 1 == NB ? 0 : st_slot + 1;
+    if (++sb == NB) sb = 0;
+  }
+  output(prev, epi_prev, prev_rem);
+}
+
+template <int NKS, int AXIS, int EPI>
+int launch_wide(const MmaArgs &a, const double *taps_host, cudaStream_t stream) {
+  constexpr int RR = 16 * (NKS + 1);
+  constexpr int kWarpDoubles = AXIS == 1 ? RR * 36 : 16 * (2 * RR + 8);
+  constexpr size_t smem = 4 * kWarpDoubles * sizeof(double);
+  WideTaps<NKS> taps;
+  for (int i = 0; i < 16 * NKS; ++i) taps.k[i] = i < a.ntaps ? taps_host[i] : 0.0;
+  dim3 grid;
+  if (AXIS == 1) grid = dim3((a.width + 31) / 32, (a.height + a.strip - 1) / a.strip);
+  else grid = dim3((a.width + a.strip - 1) / a.strip, (a.height + 31) / 32);
+  if (grid.y > 65535) return MB200_EUNSUPPORTED;
+  auto kernel = conv_mma_wide_kernel<NKS, AXIS, EPI>;
+  if (smem > 48 * 1024) cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
+  kernel<<<grid, 128, smem, stream>>>(a, taps);
+  count_launch();
+  count_family(kConvMma);
+  count_family(kConvMmaWide);
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return cuda_fail(e, "conv_mma_wide launch");
+  return MB200_OK;
+}
+
+template <int NKS>
+int launch_wide_nks(const MmaArgs &a, const double *taps_host, int axis, bool epi, cudaStream_t stream) {
+  if (axis == 0) return launch_wide<NKS, 0, 0>(a, taps_host, stream);
+  if (epi) return launch_wide<NKS, 1, 1>(a, taps_host, stream);
+  return launch_wide<NKS, 1, 0>(a, taps_host, stream);
+}
+
 template <int NKS, int AXIS, int IO, int EPI>
 int launch_one(const MmaArgs &a, const MmaTaps<NKS> &taps, int minb, cudaStream_t stream) {
   constexpr int NB = (4 * NKS - 8) / 8 + 2, RR = 8 * NB;
@@ -414,7 +743,12 @@ int launch_conv_mma(const void *src, void *dst, size_t width, size_t height, int
   if (epi) { a.aux = epilogue->source; a.gain = epilogue->gain; a.qthreshold = epilogue->quantum_threshold; }
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   int rc;
-  if (ntaps <= 9) rc = launch_nks<4>(a, taps, axis, io, epi, knobs.mma_minb, s);
+  // The wide tiles for windows of 18-33 taps (DESIGN §5.1); shorter windows keep the 8x8x4 tiles, since 47-72 % of a
+  // 16-row band tile would be zeros.  Wide strips start at multiples of 16 so that the bits do not depend on mma_strip.
+  if (io == 0 && ntaps >= 18 && knobs.mma_wide != 0) {
+    a.strip = (knobs.mma_strip + 15) & ~15;
+    rc = launch_wide_nks<3>(a, taps, axis, epi, s);
+  } else if (ntaps <= 9) rc = launch_nks<4>(a, taps, axis, io, epi, knobs.mma_minb, s);
   else if (ntaps <= 17) rc = launch_nks<6>(a, taps, axis, io, epi, knobs.mma_minb, s);
   else if (ntaps <= 25) rc = launch_nks<8>(a, taps, axis, io, epi, knobs.mma_minb, s);
   else rc = launch_nks<10>(a, taps, axis, io, epi, knobs.mma_minb, s);

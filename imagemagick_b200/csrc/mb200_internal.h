@@ -23,7 +23,7 @@ void count_launch(unsigned n = 1);
 // Initialised from the environment (an invalid value falls back to the default), settable with
 // mb200_set_option("<name>").  Callers take a snapshot per call.
 struct TuningKnobs {
-  int mma_strip, mma_minb, mma_l2pf, conv_mma;                        // conv_mma.cu
+  int mma_strip, mma_minb, mma_l2pf, conv_mma, mma_wide;              // conv_mma.cu
   int pair, pair_async, pair_async_col, col_rot, row_pair_rot, row_rot;   // conv1d.cu
   int resize_tma, resize_chunk, resize_slots, resize_strip;           // resize_stream.cu
   // switches (0 / 1) that force the generic paths, or opt in to a slower one, in api.cu
@@ -35,7 +35,7 @@ TuningKnobs tuning_knobs();
 
 // ---- per-family launch counters (runtime.cu): bumped where a family's kernel is launched, never on a decline -------
 enum LaunchFamily {
-  kConvMma,                                                            // conv_mma.cu
+  kConvMma, kConvMmaWide,                                              // conv_mma.cu (a wide launch counts in both)
   kConvPair, kConvPairAsync, kConvGeneric,                             // conv1d.cu
   kResizeVStream, kResizeHTma, kResizeHStream, kResizeFused,           // resize_stream.cu
   kResizeRegular, kResizeGather,                                       // resize.cu

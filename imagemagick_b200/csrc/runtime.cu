@@ -81,6 +81,8 @@ const KnobSpec kKnobs[] = {
     {"mma_l2pf", &TuningKnobs::mma_l2pf, -1, [](int v) { return v >= -1 && v <= 1; }},    // -1: windows of <= 9 taps
     // matrix path of the separable convolution: -1 automatic (float in / float out passes), 0 never, 1 whenever possible
     {"conv_mma", &TuningKnobs::conv_mma, -1, [](int v) { return v >= -1 && v <= 1; }, kInteger, "MB200_MMA"},
+    // DMMA.16x8x16 tiles on the matrix path: -1 automatic (windows of 18-33 taps), 0 never, 1 every float-in pass
+    {"mma_wide", &TuningKnobs::mma_wide, -1, [](int v) { return v >= -1 && v <= 1; }},
     {"pair", &TuningKnobs::pair, 1, [](int v) { return v == 0 || v == 1; }},
     {"pair_async", &TuningKnobs::pair_async, 1, [](int v) { return v == 0 || v == 1; }},
     {"pair_async_col", &TuningKnobs::pair_async_col, -1, [](int v) { return v >= -1 && v <= 1; }},   // -1: < 33 taps
@@ -138,7 +140,7 @@ int knob_index(const char *name) {
 }
 
 const char *const kFamilyNames[kLaunchFamilies] = {
-    "conv_mma_launches", "conv_pair_launches", "conv_pair_async_launches", "conv_generic_launches",
+    "conv_mma_launches", "conv_mma_wide_launches", "conv_pair_launches", "conv_pair_async_launches", "conv_generic_launches",
     "resize_v_stream_launches", "resize_h_tma_launches", "resize_h_stream_launches", "resize_fused_launches",
     "resize_regular_launches", "resize_gather_launches", "conv2d_dense_r8_launches", "conv2d_dense_r4_launches",
     "conv2d_dense_r2_launches", "morph2d_launches", "minmax2d_launches", "morph_stream_launches", "morph_direct_launches"};
