@@ -111,6 +111,7 @@ class Image:
             raise ValueError("1..4 channels (Gray, Gray+Alpha, RGB, RGBA), or 5 for CMYK with alpha")
         self.pixels = pixels
         self.colorspace = colorspace
+        self.page = (0, 0)                 # the virtual canvas offset (page.x, page.y) DistortImage reads and sets
 
     rows = property(lambda self: int(self.pixels.shape[0]))
     columns = property(lambda self: int(self.pixels.shape[1]))
@@ -380,6 +381,122 @@ def ResizeImage(image: Image, columns: int, rows: int, filter: int = UndefinedFi
         check(lib.mb200_resize_image_ex(image._ptr(), image.columns, image.rows, image.channels, out._ptr(), columns,
                                         rows, int(filter), ref))
     return out
+
+
+class DistortParams(C.Structure):
+    """mb200_distort_params: the reverse map and output geometry mb200_distort_plan / mb200_rotate_plan compute."""
+    _fields_ = [("map", C.c_int), ("coeff", C.c_double * 9), ("columns", C.c_size_t), ("rows", C.c_size_t),
+                ("page_x", C.c_long), ("page_y", C.c_long), ("output_scaling", C.c_double), ("bestfit", C.c_int),
+                ("src_page_x", C.c_long), ("src_page_y", C.c_long)]
+
+
+class ResampleOptions(C.Structure):
+    """mb200_resample_options: the source image's filter, virtual-pixel method, interpolate and colours."""
+    _fields_ = [("filter", C.c_int), ("filter_options", C.c_void_p), ("virtual_pixel", C.c_int),
+                ("interpolate", C.c_int), ("background", C.c_double * 4), ("matte", C.c_double * 4),
+                ("matte_alpha", C.c_int)]
+
+
+# MagickCore/distort.h DistortMethod; cache-view.h VirtualPixelMethod; pixel.h PixelInterpolateMethod
+(AffineDistortion, AffineProjectionDistortion, ScaleRotateTranslateDistortion, PerspectiveDistortion,
+ PerspectiveProjectionDistortion) = 1, 2, 3, 4, 5
+RigidAffineDistortion = 19
+(UndefinedVirtualPixelMethod, BackgroundVirtualPixelMethod, EdgeVirtualPixelMethod, TransparentVirtualPixelMethod,
+ BlackVirtualPixelMethod, GrayVirtualPixelMethod, WhiteVirtualPixelMethod) = 0, 1, 3, 7, 9, 10, 11
+UndefinedInterpolatePixel, BilinearInterpolatePixel = 0, 5
+WHITE = (65535.0, 65535.0, 65535.0)                      # BackgroundColorRGBA (image-private.h:32)
+MATTE = (48573.0, 48573.0, 48573.0)                      # MatteColorRGBA #BDBDBD (image-private.h:56)
+
+
+def DistortPlan(image: Image, method: int, arguments, bestfit: bool = False, viewport=None,
+                scale: Optional[float] = None) -> DistortParams:
+    """GenerateCoefficients and the output geometry of MagickCore/distort.c:1754 for the affine and perspective methods,
+    on the host.  viewport: (width, height, x, y), the "distort:viewport" geometry; scale: "distort:scale"."""
+    args = (C.c_double * max(1, len(arguments)))(*[float(a) for a in arguments])
+    vp = (C.c_long * 4)(*[int(v) for v in viewport]) if viewport is not None else None
+    plan = DistortParams()
+    page = getattr(image, "page", (0, 0))
+    check(_lib.load().mb200_distort_plan(int(method), args, len(arguments), int(bool(bestfit)), image.columns,
+                                         image.rows, int(page[0]), int(page[1]), vp, float("nan") if scale is None else float(scale),
+                                         C.byref(plan)))
+    return plan
+
+
+def _opaque_alpha(image: Image) -> Image:
+    """The image with an opaque alpha channel appended (Gray -> Gray+Alpha, RGB -> RGBA), page kept."""
+    if image.on_device:
+        import torch
+        a = torch.full((image.rows, image.columns, 1), 65535.0, dtype=torch.float32, device=image.pixels.device)
+        out = Image(torch.cat([image.pixels, a], dim=2), image.colorspace)
+    else:
+        out = Image(np.concatenate([image.pixels, np.full((image.rows, image.columns, 1), 65535.0, np.float32)], axis=2),
+                    image.colorspace)
+    out.page = getattr(image, "page", (0, 0))
+    return out
+
+
+def _distort(image: Image, plan: DistortParams, filter: int, virtual_pixel: int, interpolate: int, background,
+             matte_color, artifacts) -> Image:
+    if image.colorspace == CMYKColorspace:
+        raise MagickB200Error(_lib.EUNSUPPORTED, "distort: CMYK (its black channel) is not implemented")
+    bg = tuple(background) + (65535.0,) * (4 - len(background))
+    if image.channels in (1, 2) and not bg[0] == bg[1] == bg[2]:
+        raise MagickB200Error(_lib.EUNSUPPORTED, "distort: a gray image with a non-gray background becomes sRGB")
+    if image.channels in (1, 3) and len(matte_color) == 4:
+        raise MagickB200Error(_lib.EUNSUPPORTED, "distort: a matte colour with alpha adds alpha inside DistortImage")
+    if image.channels in (1, 3) and len(background) == 4 and virtual_pixel not in (BackgroundVirtualPixelMethod,
+                                                                                    TransparentVirtualPixelMethod):
+        raise MagickB200Error(_lib.EUNSUPPORTED, "distort: a background with alpha adds alpha inside DistortImage")
+    if image.channels in (1, 3) and ((len(background) == 4 and virtual_pixel == BackgroundVirtualPixelMethod) or
+                                     virtual_pixel == TransparentVirtualPixelMethod):
+        # SetImageVirtualPixelMethod(Background with alpha / Transparent) gives the source an opaque alpha channel
+        # before the reference resamples it (cache.c:5294-5309)
+        image = _opaque_alpha(image)
+    opts = ResampleOptions(filter=int(filter), virtual_pixel=int(virtual_pixel), interpolate=int(interpolate))
+    fo = filter_options_from_artifacts(artifacts)
+    opts.filter_options = C.cast(C.byref(fo), C.c_void_p) if fo is not None else None
+    opts.background[:] = [float(v) for v in bg]
+    opts.matte[:] = [float(v) for v in tuple(matte_color) + (65535.0,) * (4 - len(matte_color))]
+    opts.matte_alpha = int(len(matte_color) == 4)
+    lib = _lib.load()
+    out = image._new_like(rows=plan.rows, columns=plan.columns)
+    if image.on_device:
+        _activate(image)
+        check(lib.mb200_distort_image_dev(image._ptr(), image.columns, image.rows, image.channels, out._ptr(),
+                                          C.byref(plan), C.byref(opts), _stream(image)))
+    else:
+        check(lib.mb200_distort_image(image._ptr(), image.columns, image.rows, image.channels, out._ptr(),
+                                      C.byref(plan), C.byref(opts)))
+    out.page = (plan.page_x, plan.page_y)
+    return out
+
+
+def DistortImage(image: Image, method: int, arguments, bestfit: bool = False, *, filter: int = UndefinedFilter,
+                 virtual_pixel: int = UndefinedVirtualPixelMethod, interpolate: int = UndefinedInterpolatePixel,
+                 background=WHITE, matte_color=MATTE, viewport=None, scale: Optional[float] = None,
+                 artifacts=None) -> Image:
+    """MagickCore/distort.c:1754 with Affine, AffineProjection, ScaleRotateTranslate, RigidAffine, Perspective
+    and PerspectiveProjection, through the EWA sampler of resample.c; bit exact.  `image.page` (default (0, 0)) is read and
+    the result's page set.  filter / virtual_pixel / interpolate / background / matte_color are the source image's
+    settings (a 4-tuple colour has an alpha trait); viewport / scale are "distort:viewport" / "distort:scale" as values,
+    artifacts the "filter:*" settings.  As SetImageVirtualPixelMethod does, a Gray or RGB image gains an opaque alpha
+    channel for Transparent virtual pixels, or Background ones with a background that has an alpha trait; other
+    colours with an alpha trait on such an image (the reference adds alpha inside DistortImage), CMYK, and a Gray image with a non-gray background (the reference turns it into sRGB), raise MB200_EUNSUPPORTED."""
+    plan = DistortPlan(image, method, arguments, bestfit, viewport, scale)
+    return _distort(image, plan, filter, virtual_pixel, interpolate, background, matte_color, artifacts)
+
+
+def RotateImage(image: Image, degrees: float, background=WHITE, *, filter: int = UndefinedFilter,
+                matte_color=MATTE) -> Image:
+    """MagickCore/distort.c:2954 for angles that are not a multiple of 90 degrees (those raise MB200_EUNSUPPORTED):
+    DistortImage(ScaleRotateTranslate, bestfit) with Background virtual pixels.  A 4-tuple background has an alpha
+    trait: a Gray or RGB image then gains an opaque alpha channel, as SetImageVirtualPixelMethod gives it one."""
+    plan = DistortParams()
+    page = getattr(image, "page", (0, 0))
+    check(_lib.load().mb200_rotate_plan(float(degrees), image.columns, image.rows, int(page[0]), int(page[1]),
+                                        C.byref(plan)))
+    return _distort(image, plan, filter, BackgroundVirtualPixelMethod, UndefinedInterpolatePixel, background,
+                    matte_color, None)
 
 
 def SampleImage(image: Image, columns: int, rows: int) -> Image:

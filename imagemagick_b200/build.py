@@ -27,7 +27,9 @@ NVCC_FLAGS = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC,-fvisibilit
 
 SOURCES = ["runtime.cu", "kernel_info.cpp", "resize_filter.cpp", "resize_tables.cpp", "conv1d.cu", "conv_mma.cu",
            "morph2d.cu", "morph_stream.cu", "morph_direct.cu", "cache.cu", "resize.cu", "resize_stream.cu", "colorspace.cu", "hexcone.cu", "pointwise.cu", "equalize.cu", "stencils.cu", "hooks.cu", "enhance.cu", "layout.cu", "level.cu",
-           "api.cu"]
+           "distort_plan.cpp", "distort.cu", "api.cu"]
+# distort.cu restates the reference's EWA sampler operation by operation: no contraction into fused multiply-adds.
+FILE_FLAGS = {"distort.cu": ["-fmad=false"]}
 
 
 def _nvcc() -> str:
@@ -53,7 +55,7 @@ def build(force: bool = False, verbose: bool = False) -> Path:
         src = CSRC / name
         obj = OBJDIR / (src.stem + ".o")
         if force or _stale(obj, [src] + headers):
-            cmd = [nvcc, *ARCH, *NVCC_FLAGS, "-x", "cu", "-c", str(src), "-o", str(obj)]
+            cmd = [nvcc, *ARCH, *NVCC_FLAGS, *FILE_FLAGS.get(name, []), "-x", "cu", "-c", str(src), "-o", str(obj)]
             jobs.append((name, cmd, obj))
 
     def run(job):

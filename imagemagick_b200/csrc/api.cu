@@ -469,6 +469,16 @@ int mb200_morphology_direct_image_dev(const float *src, float *dst, size_t width
   return launch_morphology_direct(src, static_cast<float *>(tmp.ptr), dst, width, height, channels, method, kernel, s);
 }
 
+int mb200_distort_image_dev(const float *src, size_t width, size_t height, int channels, float *dst,
+                            const mb200_distort_params *plan, const mb200_resample_options *options, void *stream) {
+  if (!src || !dst || src == dst) return fail(MB200_EINVAL, "distort: bad arguments");
+  int rc = distort_check(width, height, channels, plan, options);
+  cudaStream_t s;
+  if (!rc) rc = prepare(stream, &s);
+  if (rc) return rc;
+  return launch_distort(src, width, height, channels, dst, plan, options, s);
+}
+
 int mb200_convolve_image_dev(const float *src, float *dst, size_t width, size_t height, int channels,
                              const mb200_kernel_info *kernel, void *stream) {
   return mb200_morphology_image_dev(src, dst, width, height, channels, MB200_ConvolveMorphology, 1, kernel, 0.0,
@@ -646,6 +656,16 @@ int mb200_morphology_direct_image(const float *src, float *dst, size_t w, size_t
   if (rc) return rc;
   return with_staging("morphology direct", src, w, h, ch, dst, w, h, [&](const float *s, float *d, cudaStream_t st) {
     return mb200_morphology_direct_image_dev(s, d, w, h, ch, method, kernel, st);
+  });
+}
+
+int mb200_distort_image(const float *src, size_t w, size_t h, int ch, float *dst, const mb200_distort_params *plan,
+                        const mb200_resample_options *options) {
+  if (!src || !dst) return fail(MB200_EINVAL, "distort: bad arguments");
+  const int rc = distort_check(w, h, ch, plan, options);
+  if (rc) return rc;
+  return with_staging("distort", src, w, h, ch, dst, plan->columns, plan->rows, [&](const float *s, float *d, cudaStream_t st) {
+    return mb200_distort_image_dev(s, w, h, ch, d, plan, options, st);
   });
 }
 

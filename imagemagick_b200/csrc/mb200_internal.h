@@ -42,6 +42,7 @@ enum LaunchFamily {
   kConv2dDenseR8, kConv2dDenseR4, kConv2dDenseR2, kMorph2d, kMinmax2d, // morph2d.cu
   kMorphStream,                                                        // morph_stream.cu
   kMorphDirect,                                                        // morph_direct.cu
+  kDistort,                                                            // distort.cu
   kLaunchFamilies
 };
 void count_family(LaunchFamily family);
@@ -127,6 +128,13 @@ int launch_morph_stream(const float *src, float *dst, size_t width, size_t heigh
 int morphology_direct_check(int channels, int method, const mb200_kernel_info *kernel);
 int launch_morphology_direct(const float *src, float *tmp, float *dst, size_t width, size_t height, int channels,
                              int method, const mb200_kernel_info *kernel, void *stream);
+
+// distort.cu: DistortImage's sampling loop for a plan of distort_plan.cpp.  The check runs on the host before anything
+// is touched (MB200_EINVAL / MB200_EUNSUPPORTED as documented at mb200_distort_image_dev); the launch is one kernel.
+int distort_check(size_t width, size_t height, int channels, const mb200_distort_params *plan,
+                  const mb200_resample_options *options);
+int launch_distort(const float *src, size_t width, size_t height, int channels, float *dst,
+                   const mb200_distort_params *plan, const mb200_resample_options *options, void *stream);
 
 // ---- resize axis tables (resize_tables.cpp) ---------------------------------
 // One axis of ResizeImage, planned on the host and resident on one device: the reference's contribution lists

@@ -5,8 +5,9 @@
 // :835-876, function table :888-942, sharpening :1064, cubic coefficients :1181-1226),
 // GetResizeFilterWeight :1690, GetResizeFilterSupport :1656, and the contribution
 // set-up that opens every iteration of HorizontalFilter (:3398-3443) and
-// VerticalFilter (:3614-3657).  No "filter:*" artifacts (the shim declines when any
-// is set), never cylindrical (ResizeImage passes MagickFalse, :3817).
+// VerticalFilter (:3614-3657).  Orthogonal for ResizeImage (MagickFalse, :3817);
+// cylindrical (:995-997, :1033, :1049-1069) for the EWA weight table of
+// SetResampleFilter (resample.c:1246-1300), which DistortImage samples through.
 //
 // Weights are evaluated on the host in double with the same operation order as the
 // reference, so the table uploaded to the GPU is bit-identical to what the CPU path
@@ -101,12 +102,15 @@ struct ResizeFilter {
 
   // The expert settings take effect in the reference's order (resize.c:999-1226): window override, sharpening, Gaussian
   // sigma (widens the support), Kaiser beta, lobes, Jinc zeros, blur, support, window support, window scale, cubic B / C.
-  explicit ResizeFilter(int requested, const mb200_filter_options *opt = nullptr) {
+  explicit ResizeFilter(int requested, const mb200_filter_options *opt = nullptr, bool cylindrical = false) {
     if (requested <= MB200_UndefinedFilter || requested >= MB200_SentinelFilter) return;
     const unsigned set = opt ? opt->set : 0u;
     int ft = kMapping[requested].filter, wt = kMapping[requested].window;
+    if (cylindrical && ft == MB200_SincFastFilter && requested != MB200_SincFastFilter)
+      ft = MB200_JincFilter;                                 // 1-D windowed Sinc => 2-D windowed Jinc (:995-997)
     if ((set & MB200_FO_WINDOW) && opt->window > MB200_UndefinedFilter && opt->window < MB200_SentinelFilter) {
-      if (!opt->keep_filter) ft = MB200_SincFastFilter;     // a window without a filter: windowed Sinc (:1024-1041)
+      // a window without a filter: windowed Sinc, or Jinc when cylindrical (:1024-1041)
+      if (!opt->keep_filter) ft = cylindrical ? MB200_JincFilter : MB200_SincFastFilter;
       wt = opt->window;
     }
     filter = kFunctions[ft].fn;
@@ -114,6 +118,14 @@ struct ResizeFilter {
     if (filter == Fn::Unsupported || window == Fn::Unsupported) return;
     support = kFunctions[ft].support;
     scale = kFunctions[wt].scale;
+    if (cylindrical) {                                       // :1049-1069
+      if (ft == MB200_BoxFilter) support = 0.70710678118654752440;      // MagickSQ1_2
+      if (ft == MB200_LanczosFilter || ft == MB200_LanczosSharpFilter || ft == MB200_Lanczos2Filter ||
+          ft == MB200_Lanczos2SharpFilter || ft == MB200_LanczosRadiusFilter) {
+        filter = window = Fn::Jinc;
+        scale = kFunctions[MB200_JincFilter].scale;
+      }
+    }
     if (ft == MB200_LanczosSharpFilter) blur *= 0.9812505644269356;
     if (ft == MB200_Lanczos2SharpFilter) blur *= 0.9549963639785485;
     if (filter == Fn::Gaussian || window == Fn::Gaussian) {
@@ -129,7 +141,10 @@ struct ResizeFilter {
       coefficient[1] = perceptible_reciprocal(bessel_i0(beta));
     }
     if (set & MB200_FO_LOBES) support = static_cast<double>(opt->lobes < 1 ? 1 : opt->lobes);   // :1123-1133
-    if (filter == Fn::Jinc) support = jinc_zero(static_cast<long>(support));   // :1135-1150 lobes -> support
+    if (filter == Fn::Jinc) {                                // :1135-1150 lobes -> support
+      support = jinc_zero(static_cast<long>(support));
+      if (ft == MB200_LanczosRadiusFilter) blur *= std::floor(support) / support;
+    }
     if (set & MB200_FO_BLUR) blur *= opt->blur;              // :1155-1157
     if (blur < kEps) blur = kEps;
     if (set & MB200_FO_SUPPORT) support = std::fabs(opt->support);             // :1163-1165
@@ -321,6 +336,21 @@ double mb200_resize_filter_support_ex(int filter, const mb200_filter_options *op
   return rf.practical_support();
 }
 double mb200_resize_filter_support(int filter) { return mb200_resize_filter_support_ex(filter, nullptr); }
+
+// SetResampleFilter (resample.c:1246-1300): the cylindrical filter of the image's FilterType (Undefined is Robidoux,
+// :1261) sampled at sqrt(Q) * support / sqrt(1024) for the Q = 0..1023 of the EWA's squared-radius index.
+int mb200_resample_filter_lut(int filter, const mb200_filter_options *options, double *lut, double *support) {
+  if (filter == MB200_UndefinedFilter) filter = MB200_RobidouxFilter;
+  if (filter == MB200_PointFilter)
+    return mb200::fail(MB200_EUNSUPPORTED, "the Point filter interpolates every pixel instead of sampling an ellipse");
+  ResizeFilter rf(filter, options, true);
+  if (!rf.valid) return mb200::fail(MB200_EINVAL, "resample filter %d is not a FilterType", filter);
+  if (!lut || !support) return mb200::fail(MB200_EINVAL, "resample filter: no output");
+  *support = rf.practical_support();
+  const double r_scale = *support * std::sqrt(1.0 / static_cast<double>(MB200_RESAMPLE_LUT));
+  for (int q = 0; q < MB200_RESAMPLE_LUT; ++q) lut[q] = rf.weight(std::sqrt(static_cast<double>(q)) * r_scale);
+  return MB200_OK;
+}
 
 long mb200_resize_contributions(int filter, size_t in_n, size_t out_n, double factor, long *start,
                                 int *count, double *weights, size_t max_taps) {

@@ -29,6 +29,7 @@
 #include "MagickCore/string-private.h"          /* StringToDoubleInterval (convolve:bias, morphology.c:4163) */
 #include "MagickCore/colorspace-private.h"      /* IssRGBCompatibleColorspace (ModulateImage, enhance.c:3681) */
 #include "magick_b200.h"
+#include <math.h>
 #include <string.h>
 
 #if !defined(MAGICKCORE_HDRI_SUPPORT) || (MAGICKCORE_QUANTUM_DEPTH != 16)
@@ -38,7 +39,8 @@
 /* ---- eligibility: mirrors checkAccelerateCondition (accelerate.c:110-170) + SURVEY 8b --------- */
 /* update_mask == NULL: every channel must carry its default traits (no `-channel` selection).  Otherwise unselected
    channels (Copy trait, pixel.c:6338-6393 SetPixelChannelMask) are accepted and reported: bit c set = channel c is updated. */
-static int b200_channels_masked(const Image *image, unsigned *update_mask)
+/* The channel layout test alone, whatever the virtual-pixel method (DistortImage serves several). */
+static int b200_layout_masked(const Image *image, unsigned *update_mask)
 {
   const size_t n = GetPixelChannels(image);
   const MagickBooleanType gray = (image->colorspace == GRAYColorspace) ||
@@ -46,8 +48,6 @@ static int b200_channels_masked(const Image *image, unsigned *update_mask)
   if (image->storage_class != DirectClass) return 0;
   if ((image->channels & (ReadMaskChannel | WriteMaskChannel | CompositeMaskChannel)) != 0) return 0;
   if (image->number_meta_channels != 0) return 0;
-  if ((GetImageVirtualPixelMethod(image) != UndefinedVirtualPixelMethod) &&
-      (GetImageVirtualPixelMethod(image) != EdgeVirtualPixelMethod)) return 0;
   if (image->progress_monitor != (MagickProgressMonitor) NULL) return 0;
   if (n < 1 || n > 4) return 0;
   if (GetPixelChannelOffset(image, RedPixelChannel) != 0) return 0;
@@ -84,6 +84,13 @@ static int b200_channels_masked(const Image *image, unsigned *update_mask)
   if (n == 4 && image->alpha_trait != UndefinedPixelTrait &&
       GetPixelChannelOffset(image, AlphaPixelChannel) == 3) return 4;
   return 0;
+}
+
+static int b200_channels_masked(const Image *image, unsigned *update_mask)
+{
+  if ((GetImageVirtualPixelMethod(image) != UndefinedVirtualPixelMethod) &&
+      (GetImageVirtualPixelMethod(image) != EdgeVirtualPixelMethod)) return 0;
+  return b200_layout_masked(image, update_mask);
 }
 
 static int b200_channels(const Image *image) { return b200_channels_masked(image, (unsigned *) NULL); }
@@ -446,6 +453,124 @@ Image *B200AccelerateResizeImage(const Image *image, const size_t columns, const
     B200_ATTEMPT_END;
   }
   if (out != (Image *) NULL) out->type = image->type;
+  return out;
+}
+
+/* ---- DistortImage / RotateImage (distort.c:1754, :2954) -------------------------------------------------------- */
+/* The affine and perspective methods through the EWA sampler.  The output geometry comes from the library's planner;
+   "distort:viewport" is parsed with the reference's ParseAbsoluteGeometry over the geometry it overrides, and
+   "distort:scale" with StringToDouble.  A source without alpha whose result gains one inside DistortImage (a background
+   or matte colour with an alpha trait, distort.c:2436-2437 and pixel.c:232-234) is declined; RotateImage's own
+   SetImageVirtualPixelMethod adds that alpha before DistortImage, so its results are served.  NULL == declined, with
+   the caller's exception untouched. */
+static Image *b200_distort(const Image *image, const DistortMethod method, const size_t number_arguments,
+                           const double *arguments, const MagickBooleanType bestfit, ExceptionInfo *exception)
+{
+  const VirtualPixelMethod vpm = GetImageVirtualPixelMethod(image);
+  mb200_distort_params plan;
+  mb200_resample_options o;
+  mb200_filter_options fopt;
+  const Image *src = image;
+  Image *out = (Image *) NULL;
+  const char *a;
+  double scale = NAN;
+  long viewport[4];
+  int ch, viewport_given = 0;
+  (void) exception;
+  if (method != AffineDistortion && method != AffineProjectionDistortion && method != ScaleRotateTranslateDistortion &&
+      method != PerspectiveDistortion && method != PerspectiveProjectionDistortion && method != RigidAffineDistortion)
+    return (Image *) NULL;
+  if (mb200_device_count() <= 0 || b200_layout_masked(image, (unsigned *) NULL) == 0) return (Image *) NULL;
+  if (vpm != UndefinedVirtualPixelMethod && vpm != EdgeVirtualPixelMethod && vpm != BackgroundVirtualPixelMethod &&
+      vpm != TransparentVirtualPixelMethod && vpm != BlackVirtualPixelMethod && vpm != GrayVirtualPixelMethod &&
+      vpm != WhiteVirtualPixelMethod) return (Image *) NULL;
+  if (image->interpolate != UndefinedInterpolatePixel && image->interpolate != BilinearInterpolatePixel)
+    return (Image *) NULL;
+  if (image->filter == PointFilter || b200_filter_options(image, &fopt) == MagickFalse) return (Image *) NULL;
+  if (IsStringTrue(GetImageArtifact(image, "distort:verbose")) != MagickFalse) return (Image *) NULL;
+  if (IsGrayColorspace(image->colorspace) != MagickFalse && IsPixelInfoGray(&image->background_color) == MagickFalse)
+    return (Image *) NULL;                           /* the reference re-lays the result out to sRGB (:2433-2435) */
+  if (image->alpha_trait == UndefinedPixelTrait && (image->background_color.alpha_trait != UndefinedPixelTrait ||
+                                                    image->matte_color.alpha_trait != UndefinedPixelTrait))
+    return (Image *) NULL;                           /* the result gains alpha inside DistortImage (:2436-2437) */
+  a = GetImageArtifact(image, "distort:scale");
+  if (a != (const char *) NULL) scale = StringToDouble(a, (char **) NULL);
+  if (mb200_distort_plan((int) method, arguments, number_arguments, bestfit != MagickFalse ? 1 : 0, image->columns,
+                         image->rows, (long) image->page.x, (long) image->page.y, (const long *) NULL, NAN, &plan) != MB200_OK)
+    return (Image *) NULL;                           /* the reference raises its own argument errors */
+  a = GetImageArtifact(image, "distort:viewport");
+  if (a != (const char *) NULL) {
+    RectangleInfo geometry;
+    geometry.width = plan.columns; geometry.height = plan.rows; geometry.x = plan.page_x; geometry.y = plan.page_y;
+    if (ParseAbsoluteGeometry(a, &geometry) == NoValue) return (Image *) NULL;     /* the reference warns */
+    viewport[0] = (long) geometry.width; viewport[1] = (long) geometry.height;
+    viewport[2] = (long) geometry.x; viewport[3] = (long) geometry.y;
+    viewport_given = 1;
+  }
+  if (mb200_distort_plan((int) method, arguments, number_arguments, bestfit != MagickFalse ? 1 : 0, image->columns,
+                         image->rows, (long) image->page.x, (long) image->page.y,
+                         viewport_given ? viewport : (const long *) NULL, scale, &plan) != MB200_OK)
+    return (Image *) NULL;
+  (void) memset(&o, 0, sizeof(o));
+  o.filter = (int) image->filter;
+  o.filter_options = fopt.set != 0 ? &fopt : (const mb200_filter_options *) NULL;
+  o.virtual_pixel = (int) vpm;
+  o.interpolate = (int) image->interpolate;
+  o.background[0] = image->background_color.red; o.background[1] = image->background_color.green;
+  o.background[2] = image->background_color.blue; o.background[3] = image->background_color.alpha;
+  o.matte[0] = image->matte_color.red; o.matte[1] = image->matte_color.green;
+  o.matte[2] = image->matte_color.blue; o.matte[3] = image->matte_color.alpha;
+  o.matte_alpha = image->matte_color.alpha_trait != UndefinedPixelTrait ? 1 : 0;
+  {
+    B200_ATTEMPT_BEGIN;
+    ch = b200_layout_masked(src, (unsigned *) NULL);
+    if (ch != 0) {
+      const float *p = b200_cache_pixels(src, ch, attempt);
+      if (p != (const float *) NULL) out = new_result(src, plan.columns, plan.rows, attempt);
+      if (out != (Image *) NULL) {
+        Quantum *q = GetAuthenticPixels(out, 0, 0, out->columns, out->rows, attempt);
+        if (q == (Quantum *) NULL || b200_cache_pixels(out, ch, attempt) != (float *) q ||
+            mb200_distort_image(p, src->columns, src->rows, ch, (float *) q, &plan, &o) != MB200_OK ||
+            SyncAuthenticPixels(out, attempt) == MagickFalse)
+          out = DestroyImage(out);
+      }
+    }
+    B200_ATTEMPT_END;
+  }
+  if (out != (Image *) NULL) {
+    out->page.x = plan.page_x;
+    out->page.y = plan.page_y;
+  }
+  return out;
+}
+
+Image *B200AccelerateDistortImage(const Image *image, const DistortMethod method, const size_t number_arguments,
+                                  const double *arguments, const MagickBooleanType bestfit, ExceptionInfo *exception)
+{
+  return b200_distort(image, method, number_arguments, arguments, bestfit, exception);
+}
+
+/* RotateImage: integral rotations stay with the reference (IntegralRotateImage); otherwise its own clone, its own
+   SetImageVirtualPixelMethod(Background) -- which adds an opaque alpha or re-lays a gray image out as cache.c:5294-5309
+   does -- and DistortImage(ScaleRotateTranslate, bestfit) on it. */
+Image *B200AccelerateRotateImage(const Image *image, const double degrees, ExceptionInfo *exception)
+{
+  mb200_distort_params plan;
+  Image *clone, *out = (Image *) NULL;
+  (void) exception;
+  if (mb200_device_count() <= 0 || b200_layout_masked(image, (unsigned *) NULL) == 0) return (Image *) NULL;
+  if (mb200_rotate_plan(degrees, image->columns, image->rows, (long) image->page.x, (long) image->page.y, &plan) != MB200_OK)
+    return (Image *) NULL;
+  {
+    B200_ATTEMPT_BEGIN;
+    clone = CloneImage(image, 0, 0, MagickTrue, attempt);
+    if (clone != (Image *) NULL) {
+      (void) SetImageVirtualPixelMethod(clone, BackgroundVirtualPixelMethod, attempt);
+      out = b200_distort(clone, ScaleRotateTranslateDistortion, 1, &degrees, MagickTrue, attempt);
+      clone = DestroyImage(clone);
+    }
+    B200_ATTEMPT_END;
+  }
   return out;
 }
 
@@ -1432,6 +1557,23 @@ MagickBooleanType __wrap_ContrastStretchImage(Image *image, const double black_p
 {
   TRY_BOOL(B200AccelerateContrastStretchImage(image, black_point, white_point, exception));
   return __real_ContrastStretchImage(image, black_point, white_point, exception);
+}
+
+extern Image *__real_DistortImage(const Image *, const DistortMethod, const size_t, const double *, MagickBooleanType,
+                                  ExceptionInfo *);
+extern Image *__real_RotateImage(const Image *, const double, ExceptionInfo *);
+
+Image *__wrap_DistortImage(const Image *image, const DistortMethod method, const size_t number_arguments,
+                           const double *arguments, MagickBooleanType bestfit, ExceptionInfo *exception)
+{
+  TRY(B200AccelerateDistortImage(image, method, number_arguments, arguments, bestfit, exception));
+  return __real_DistortImage(image, method, number_arguments, arguments, bestfit, exception);
+}
+
+Image *__wrap_RotateImage(const Image *image, const double degrees, ExceptionInfo *exception)
+{
+  TRY(B200AccelerateRotateImage(image, degrees, exception));
+  return __real_RotateImage(image, degrees, exception);
 }
 
 MagickBooleanType __wrap_NormalizeImage(Image *image, ExceptionInfo *exception)

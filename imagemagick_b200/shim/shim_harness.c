@@ -178,6 +178,33 @@ static int level_case(const char *name, int bar, const Image *src, int op, doubl
   return bad || d > bar;
 }
 
+/* DistortImage (method >= 0) / RotateImage (method < 0) on `src` through the shim and through __real_: pixels (bit
+   exact), size, page and channel count must agree; with `expect_fallback` the shim must have declined.  1 on failure. */
+extern Image *__real_DistortImage(const Image *, const DistortMethod, const size_t, const double *, MagickBooleanType,
+                                  ExceptionInfo *);
+extern Image *__real_RotateImage(const Image *, const double, ExceptionInfo *);
+static int distort_case(const char *name, const Image *src, int method, size_t n, const double *args,
+                        MagickBooleanType bestfit, int expect_fallback, ExceptionInfo *ex)
+{
+  const long fb = B200ShimFallbacks();
+  Image *a, *b;
+  long d = 0;
+  int bad = 0;
+  a = method < 0 ? RotateImage(src, args[0], ex) : DistortImage(src, (DistortMethod) method, n, args, bestfit, ex);
+  B200ShimEnable(0);
+  b = method < 0 ? __real_RotateImage(src, args[0], ex) : __real_DistortImage(src, (DistortMethod) method, n, args, bestfit, ex);
+  B200ShimEnable(1);
+  if (!a || !b || GetPixelChannels(a) != GetPixelChannels(b) || a->page.x != b->page.x || a->page.y != b->page.y) bad = 1;
+  else d = compare(a, b, ex);
+  if (expect_fallback && mb200_device_count() > 0 && B200ShimFallbacks() <= fb) bad = 1;
+  if (!expect_fallback && mb200_device_count() > 0 && B200ShimFallbacks() > fb) bad = 1;
+  printf("%-34s max ULP %ld (bar 0) channels %d/%d%s\n", name, d, a ? (int) GetPixelChannels(a) : 0,
+         b ? (int) GetPixelChannels(b) : 0, bad || d > 0 ? "  FAIL" : "");
+  if (a) a = DestroyImage(a);
+  if (b) b = DestroyImage(b);
+  return bad || d > 0;
+}
+
 int main(void)
 {
   ExceptionInfo *ex;
@@ -189,6 +216,37 @@ int main(void)
   rgba = noise_image(517, 389, MagickTrue, ex);
   rgb = noise_image(300, 200, MagickFalse, ex);
 
+  {
+    static const double srt[] = {0.8, 30.0}, rot30[] = {30.0}, rot90[] = {90.0}, polar_args[] = {20.0};
+    static const double persp[] = {0, 0, 10, 5, 516, 0, 480, 30, 0, 388, 20, 360, 516, 388, 500, 380};
+    /* Fresh images: a clone shares its pixel cache, and with it the virtual-pixel method, which RotateImage sets to
+       Background on its clone (as the reference does), so a clone of rgba would change rgba for the cases below. */
+    Image *rot = noise_image(517, 389, MagickTrue, ex), *persp4 = noise_image(517, 389, MagickTrue, ex);
+    Image *none = noise_image(300, 200, MagickFalse, ex), *none2 = noise_image(300, 200, MagickFalse, ex);
+    Image *g = noise_image(300, 200, MagickFalse, ex), *gray = converted(g, GRAYColorspace, ex);
+    Image *point = noise_image(64, 48, MagickTrue, ex), *tile = noise_image(64, 48, MagickTrue, ex);
+    Image *polar = noise_image(64, 48, MagickTrue, ex), *r90 = noise_image(64, 48, MagickTrue, ex);
+    Image *c = noise_image(64, 48, MagickFalse, ex), *cmyk = converted(c, CMYKColorspace, ex);
+    (void) QueryColorCompliance("none", AllCompliance, &none->background_color, ex);
+    (void) QueryColorCompliance("none", AllCompliance, &none2->background_color, ex);
+    point->filter = PointFilter;
+    (void) SetImageVirtualPixelMethod(tile, TileVirtualPixelMethod, ex);
+    failures += distort_case("RotateImage 30 RGBA", rot, -1, 1, rot30, MagickTrue, 0, ex);
+    failures += distort_case("RotateImage 30 RGB -background none", none, -1, 1, rot30, MagickTrue, 0, ex);
+    failures += distort_case("fallback: DistortImage SRT RGB -background none", none2, ScaleRotateTranslateDistortion,
+                             2, srt, MagickTrue, 1, ex);
+    failures += distort_case("RotateImage 30 gray", gray, -1, 1, rot30, MagickTrue, 0, ex);
+    failures += distort_case("DistortImage Perspective RGBA", persp4, PerspectiveDistortion, 16, persp, MagickTrue, 0, ex);
+    failures += distort_case("fallback: DistortImage Point filter", point, ScaleRotateTranslateDistortion, 2, srt,
+                             MagickTrue, 1, ex);
+    failures += distort_case("fallback: DistortImage Tile", tile, ScaleRotateTranslateDistortion, 2, srt, MagickTrue, 1, ex);
+    failures += distort_case("fallback: DistortImage Polar", polar, PolarDistortion, 1, polar_args, MagickTrue, 1, ex);
+    failures += distort_case("fallback: RotateImage 90", r90, -1, 1, rot90, MagickTrue, 1, ex);
+    failures += distort_case("fallback: RotateImage CMYK", cmyk, -1, 1, rot30, MagickTrue, 1, ex);
+    rot = DestroyImage(rot); persp4 = DestroyImage(persp4); none = DestroyImage(none); none2 = DestroyImage(none2);
+    g = DestroyImage(g); gray = DestroyImage(gray); point = DestroyImage(point); tile = DestroyImage(tile);
+    polar = DestroyImage(polar); r90 = DestroyImage(r90); c = DestroyImage(c); cmyk = DestroyImage(cmyk);
+  }
   CHECK("BlurImage(0,4) RGBA", 1, BlurImage(rgba, 0.0, 4.0, ex), CPU(__real_BlurImage(rgba, 0.0, 4.0, ex)));
   CHECK("BlurImage(0,2) RGB", 1, BlurImage(rgb, 0.0, 2.0, ex), CPU(__real_BlurImage(rgb, 0.0, 2.0, ex)));
   CHECK("GaussianBlurImage(0,1.5) RGBA", 1, GaussianBlurImage(rgba, 0.0, 1.5, ex), CPU(__real_GaussianBlurImage(rgba, 0.0, 1.5, ex)));

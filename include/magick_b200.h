@@ -300,6 +300,49 @@ MB200_API double mb200_resize_filter_support_ex(int filter, const mb200_filter_o
 MB200_API double mb200_resize_filter_weight(int filter, double x);
 MB200_API double mb200_resize_filter_support(int filter);
 
+/* ---- DistortImage / RotateImage (MagickCore/distort.c:1754, :2954) through resample.c's EWA sampler ----
+   The planner runs on the host without a device: GenerateCoefficients (distort.c:380-960) for Affine (1),
+   AffineProjection (2), ScaleRotateTranslate (3), Perspective (4), PerspectiveProjection (5) and RigidAffine (19) --
+   all reduce to an affine (6 coefficients) or a perspective (9) reverse map -- and the output geometry: bestfit
+   bounds (:1827-1990), a "distort:viewport" given as values, and "distort:scale" (:2393-2410, NaN = not set).  The
+   caller allocates dst from plan->columns x plan->rows.  MB200_EUNSUPPORTED: another method; MB200_EINVAL: the
+   reference's argument errors (too few / many arguments, a zero scale, an unsolvable matrix, a scale below 0.1). */
+#define MB200_RESAMPLE_LUT 1024
+typedef enum { MB200_DistortAffineMap = 0, MB200_DistortPerspectiveMap = 1 } mb200_distort_map;
+typedef struct mb200_distort_params {
+  int map;                       /* mb200_distort_map */
+  double coeff[9];               /* output -> source: affine c0..c5; perspective c0..c7 and the ground sign c8 */
+  size_t columns, rows;          /* the output image */
+  long page_x, page_y;           /* the output's page offset (geometry.x / y) */
+  double output_scaling;         /* 1 / |distort:scale| */
+  int bestfit;                   /* the source's page is subtracted from each sample point (:2853-2856) */
+  long src_page_x, src_page_y;
+} mb200_distort_params;
+MB200_API int mb200_distort_plan(int method, const double *arguments, size_t number_arguments, int bestfit,
+    size_t width, size_t height, long page_x, long page_y, const long *viewport /* w, h, x, y or NULL */,
+    double scale, mb200_distort_params *plan);
+/* RotateImage's angle reduction (:2976-2988); MB200_EUNSUPPORTED where the reference takes IntegralRotateImage. */
+MB200_API int mb200_rotate_plan(double degrees, size_t width, size_t height, long page_x, long page_y,
+    mb200_distort_params *plan);
+
+/* The source image's resample settings.  filter: its FilterType (Undefined = Robidoux; Point is MB200_EUNSUPPORTED,
+   it interpolates every pixel); filter_options: "filter:*" settings or NULL; virtual_pixel: Undefined (0),
+   Background (1), Edge (3), Transparent (7), Black (9), Gray (10), White (11); interpolate: Undefined (0) or
+   Bilinear (5); background / matte: the colours as doubles (rgba), matte_alpha != 0 when the matte colour has an
+   alpha trait.  On a gray image the background must be gray (the reference re-lays a gray image out to sRGB
+   otherwise) and its blue component is the gray value. */
+typedef struct mb200_resample_options {
+  int filter;
+  const mb200_filter_options *filter_options;
+  int virtual_pixel;
+  int interpolate;
+  double background[4];
+  double matte[4];
+  int matte_alpha;
+} mb200_resample_options;
+/* The cylindrical weight table of SetResampleFilter (resample.c:1246-1300): lut[MB200_RESAMPLE_LUT], *support. */
+MB200_API int mb200_resample_filter_lut(int filter, const mb200_filter_options *options, double *lut, double *support);
+
 /* --------------------------------------- device-resident operators (HBM) ---- */
 /* src/dst are DEVICE pointers (from mb200_malloc or any CUDA allocation, e.g. a
    torch tensor's data_ptr()); they must not alias unless stated.  `stream` is a
@@ -337,6 +380,17 @@ MB200_API int mb200_morphology_image_dev(const float *src, float *dst, size_t wi
    beyond shared memory).  Both are checked before the device is touched. */
 MB200_API int mb200_morphology_direct_image_dev(const float *src, float *dst, size_t width, size_t height,
     int channels, int method, const mb200_kernel_info *kernel, void *stream);
+
+/* DistortImage's sampling loop (MagickCore/distort.c:2474-2890) for a plan from mb200_distort_plan /
+   mb200_rotate_plan: one thread per output pixel runs the map, the perspective validity and horizon blend, and
+   ResamplePixelColor (resample.c:315-670) -- the miss test, the limit fallbacks, the EWA parallelogram scan over the
+   weight table and the interpolated fallback -- in the reference's order with unfused double operations: bit exact.
+   dst (plan->columns x plan->rows x channels) must not alias src.  MB200_EUNSUPPORTED, before the device is touched
+   and with dst untouched: the Point filter, interpolate methods other than Undefined / Bilinear, virtual-pixel
+   methods other than the six above, and a perspective map on an image without alpha whose horizon blend band
+   crosses the output (the reference's blend there reads an alpha sum carried along the row). */
+MB200_API int mb200_distort_image_dev(const float *src, size_t width, size_t height, int channels, float *dst,
+    const mb200_distort_params *plan, const mb200_resample_options *options, void *stream);
 
 /* ConvolveImage (MagickCore/effect.c:1170) */
 MB200_API int mb200_convolve_image_dev(const float *src, float *dst, size_t width, size_t height,
@@ -595,6 +649,8 @@ MB200_API int mb200_morphology_direct_image(const float *src, float *dst, size_t
     int channels, int method, const mb200_kernel_info *kernel);
 MB200_API int mb200_unsharp_mask_image(const float *src, float *dst, size_t width, size_t height,
     int channels, double radius, double sigma, double gain, double threshold);
+MB200_API int mb200_distort_image(const float *src, size_t width, size_t height, int channels, float *dst,
+    const mb200_distort_params *plan, const mb200_resample_options *options);
 MB200_API int mb200_sharpen_image(const float *src, float *dst, size_t width, size_t height, int channels,
     double radius, double sigma);
 MB200_API int mb200_edge_image(const float *src, float *dst, size_t width, size_t height, int channels,

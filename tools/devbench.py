@@ -1,5 +1,6 @@
 """Developer micro-benchmark: device-resident timings of the hot-path operators (CUDA events).
-usage: python tools/devbench.py [blur|resize|lab|dilate|erode|gauss|conv2d|stencils|hooks|enhance|layout|level|direct|all] [size]"""
+usage: python tools/devbench.py [blur|resize|lab|dilate|erode|gauss|conv2d|stencils|hooks|enhance|layout|level|direct|distort|all]
+       [size] [ref]   (ref: distort also times the reference's all-core DistortImage / RotateImage, minutes at 8192^2)"""
 import sys
 from pathlib import Path
 sys.path.insert(0, str(Path(__file__).resolve().parent.parent))
@@ -236,5 +237,56 @@ if which in ("direct", "all"):
                                            4, method, ctypes.c_long(1), ctypes.c_char_p(kernel.encode()), ctypes.byref(trait))
             t = time.perf_counter() - t0
             line += f"  reference 1 thread {t * 1e3:9.1f} ms (rc {rc})"
+        print(line, flush=True)
+    del x
+
+if which in ("distort", "all"):
+    # DistortImage / RotateImage at size^2 RGBA, device-resident, with the card and its power limit.  Floor: 16 B/px
+    # read + 16 B/px written per output pixel at the 3.35 TB/s H100 SXM data-sheet HBM bandwidth (the source is read
+    # about once when the ellipse covers ~1 source pixel per output pixel).  With "ref", the reference itself runs on
+    # all cores on the same image (oracle/_ref).
+    import ctypes
+    import subprocess
+    import time
+    import numpy as np
+    DATASHEET = 3350.0
+    try:
+        limit = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i",
+                                str(torch.cuda.current_device())], capture_output=True, text=True, timeout=30).stdout.strip()
+    except (OSError, subprocess.SubprocessError):
+        limit = "unknown"
+    print(f"DistortImage on {torch.cuda.get_device_name()} at a power limit of {limit or 'unknown'}", flush=True)
+    with_ref = len(sys.argv) > 3 and sys.argv[3] == "ref"
+    ref_so = Path(__file__).resolve().parent.parent / "oracle" / "_ref" / "libmagickref_distort.so"
+    ref = ctypes.CDLL(str(ref_so)) if with_ref and ref_so.exists() else None
+    src = torch.rand(size, size, 4, device="cuda") * 65535
+    x = im.Image(src)
+    host = src.cpu().numpy()
+    c = float(size)
+    cases = [("RotateImage 30", 0, [30.0], True),
+             ("SRT 0.5x 30deg", im.ScaleRotateTranslateDistortion, [0.5, 30.0], True),
+             ("Affine 2x", im.AffineDistortion, [0, 0, 0, 0, c, 0, 2 * c, 0, 0, c, 0, 2 * c], True),
+             ("Perspective with horizon", im.PerspectiveProjectionDistortion, [1.0, 0.3, 0.0, 0.0, 1.0, 0.0, 0.0, -0.6 / c],
+              False)]
+    for name, method, args, bestfit in cases:
+        fn = (lambda: im.RotateImage(x, args[0])) if method == 0 else (lambda: im.DistortImage(x, method, args, bestfit))
+        out = fn()
+        npix = out.columns * out.rows
+        ms = timeit(fn, iters=5)
+        floor = npix * 32 / DATASHEET / 1e6
+        line = (f"{name:26s} -> {out.columns}x{out.rows}  {ms:9.3f} ms  {npix / ms / 1e3:9.1f} Mpix/s  "
+                f"floor {floor:6.3f} ms = {floor / ms * 100:5.2f}%")
+        if ref is not None:
+            buf = np.empty(npix * 4 + (1 << 22), np.float32)
+            g = (ctypes.c_long * 4)()
+            d = (ctypes.c_double * len(args))(*args)
+            bg = (ctypes.c_double * 4)(65535.0, 65535.0, 65535.0, 65535.0)
+            mt = (ctypes.c_double * 4)(48573.0, 48573.0, 48573.0, 65535.0)
+            t0 = time.perf_counter()
+            rc = ref.ref_distort(ctypes.c_void_p(host.ctypes.data), ctypes.c_size_t(size), ctypes.c_size_t(size), 4,
+                                 ctypes.c_long(0), ctypes.c_long(0), method, d, ctypes.c_size_t(len(args)), int(bestfit),
+                                 0, 0, 0, bg, 0, mt, 0, None, ctypes.c_void_p(buf.ctypes.data),
+                                 ctypes.c_size_t(buf.size), g)
+            line += f"  reference all cores {(time.perf_counter() - t0) * 1e3:9.1f} ms (rc {rc})"
         print(line, flush=True)
     del x
