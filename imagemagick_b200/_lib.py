@@ -89,6 +89,9 @@ PROTOTYPES = {
     "mb200_distort_image": (_i, [_vp, _sz, _sz, _i, _vp, _vp, _vp]),
     "mb200_distort_plan": (_i, [_i, _vp, _sz, _i, _sz, _sz, _l, _l, _vp, _d, _vp]),
     "mb200_rotate_plan": (_i, [_d, _sz, _sz, _l, _l, _vp]),
+    "mb200_geometry_plan": (_i, [_i, _sz, _sz, _vp, _vp, _vp]),
+    "mb200_geometry_image_dev": (_i, [_vp, _sz, _sz, _i, _vp, _vp, _vp]),
+    "mb200_geometry_image": (_i, [_vp, _sz, _sz, _i, _vp, _vp]),
     "mb200_resample_filter_lut": (_i, [_i, _vp, _vp, _vp]),
     "mb200_convolve_image_dev": (_i, [_vp, _vp, _sz, _sz, _i, KernelPtr, _vp]),
     "mb200_blur_image_dev": (_i, [_vp, _vp, _sz, _sz, _i, _d, _d, _vp]),

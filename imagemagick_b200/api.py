@@ -21,6 +21,10 @@ include/magick_b200.h:
     LevelImage, LevelizeImage, GammaImage                           enhance.c:2913/3062/2322
     AutoLevelImage, MinMaxStretchImage                              enhance.c:187, histogram.c:927
     ContrastStretchImage, NormalizeImage, LinearStretchImage        enhance.c:1544/4130/3347
+    DistortImage, RotateImage                                       distort.c:1754/2954
+    CropImage, ShaveImage, RollImage, AutoOrientImage               transform.c:542/1641/1546/103
+    FlipImage, FlopImage, TransposeImage, TransverseImage           transform.c:1194/1329/2127/2265
+    IntegralRotateImage                                             shear.c:700
 
 An `Image` wraps the pixel cache: an (rows, columns, channels) float32 array of raw
 Quantum values (0..65535), either a NumPy array (host; every call stages through
@@ -112,6 +116,7 @@ class Image:
         self.pixels = pixels
         self.colorspace = colorspace
         self.page = (0, 0)                 # the virtual canvas offset (page.x, page.y) DistortImage reads and sets
+        self.page_size = (0, 0)            # the virtual canvas size (page.width, page.height); 0 = not set
 
     rows = property(lambda self: int(self.pixels.shape[0]))
     columns = property(lambda self: int(self.pixels.shape[1]))
@@ -497,6 +502,107 @@ def RotateImage(image: Image, degrees: float, background=WHITE, *, filter: int =
                                         C.byref(plan)))
     return _distort(image, plan, filter, BackgroundVirtualPixelMethod, UndefinedInterpolatePixel, background,
                     matte_color, None)
+
+
+class Page(C.Structure):
+    """mb200_page: an image's RectangleInfo page."""
+    _fields_ = [("width", C.c_size_t), ("height", C.c_size_t), ("x", C.c_long), ("y", C.c_long)]
+
+
+class GeometryParams(C.Structure):
+    """mb200_geometry_params: the output geometry, page and map mb200_geometry_plan computes."""
+    _fields_ = [("map", C.c_int), ("columns", C.c_size_t), ("rows", C.c_size_t), ("page", Page),
+                ("src_x", C.c_long), ("src_y", C.c_long), ("roll_x", C.c_long), ("roll_y", C.c_long)]
+
+
+# mb200_geometry_op (include/magick_b200.h)
+(GeometryCrop, GeometryShave, GeometryFlip, GeometryFlop, GeometryTranspose, GeometryTransverse,
+ GeometryIntegralRotate, GeometryRoll) = range(8)
+# MagickCore/image.h OrientationType
+(UndefinedOrientation, TopLeftOrientation, TopRightOrientation, BottomRightOrientation, BottomLeftOrientation,
+ LeftTopOrientation, RightTopOrientation, RightBottomOrientation, LeftBottomOrientation) = range(9)
+
+
+def GeometryPlan(image: Image, op: int, arguments=()) -> GeometryParams:
+    """The output geometry, page and map of one orientation or crop operator, on the host (mb200_geometry_plan).
+    `image.page` and `image.page_size` are the source's page."""
+    page = Page(*getattr(image, "page_size", (0, 0)), *getattr(image, "page", (0, 0)))
+    args = (C.c_long * 4)(*[int(a) for a in arguments])
+    plan = GeometryParams()
+    check(_lib.load().mb200_geometry_plan(int(op), image.columns, image.rows, C.byref(page), args, C.byref(plan)))
+    return plan
+
+
+def _geometry(image: Image, op: int, arguments=()) -> Image:
+    plan = GeometryPlan(image, op, arguments)
+    lib = _lib.load()
+    out = image._new_like(rows=plan.rows, columns=plan.columns)
+    if image.on_device:
+        _activate(image)
+        check(lib.mb200_geometry_image_dev(image._ptr(), image.columns, image.rows, image.channels, out._ptr(),
+                                           C.byref(plan), _stream(image)))
+    else:
+        check(lib.mb200_geometry_image(image._ptr(), image.columns, image.rows, image.channels, out._ptr(),
+                                       C.byref(plan)))
+    out.page = (plan.page.x, plan.page.y)
+    out.page_size = (plan.page.width, plan.page.height)
+    return out
+
+
+def CropImage(image: Image, width: int, height: int, x: int = 0, y: int = 0) -> Image:
+    """MagickCore/transform.c:542 with the geometry WxH+X+Y (0 = the page's width / height), against the image's page;
+    bit exact.  A crop outside the virtual canvas or of zero area raises MB200_EUNSUPPORTED (the reference warns and
+    returns a transparent 1x1 image or none)."""
+    return _geometry(image, GeometryCrop, (width, height, x, y))
+
+
+def ShaveImage(image: Image, width: int, height: int) -> Image:
+    """MagickCore/transform.c:1641; shaving half the image or more raises MB200_EUNSUPPORTED, as the reference warns."""
+    return _geometry(image, GeometryShave, (width, height))
+
+
+def FlipImage(image: Image) -> Image:
+    """MagickCore/transform.c:1194: the rows in reverse order."""
+    return _geometry(image, GeometryFlip)
+
+
+def FlopImage(image: Image) -> Image:
+    """MagickCore/transform.c:1329: the columns in reverse order."""
+    return _geometry(image, GeometryFlop)
+
+
+def TransposeImage(image: Image) -> Image:
+    """MagickCore/transform.c:2127: mirrored along the top-left to bottom-right diagonal."""
+    return _geometry(image, GeometryTranspose)
+
+
+def TransverseImage(image: Image) -> Image:
+    """MagickCore/transform.c:2265: mirrored along the bottom-left to top-right diagonal."""
+    return _geometry(image, GeometryTransverse)
+
+
+def IntegralRotateImage(image: Image, rotations: int) -> Image:
+    """MagickCore/shear.c:700: `rotations` quarter turns clockwise, taken mod 4 (as a size_t: -1 is 3).  0 raises
+    MB200_EUNSUPPORTED: the reference returns a clone."""
+    return _geometry(image, GeometryIntegralRotate, (rotations,))
+
+
+def RollImage(image: Image, x_offset: int, y_offset: int) -> Image:
+    """MagickCore/transform.c:1546: the image shifted by (x_offset, y_offset), wrapping around its edges."""
+    return _geometry(image, GeometryRoll, (x_offset, y_offset))
+
+
+def AutoOrientImage(image: Image, orientation: int) -> Image:
+    """MagickCore/transform.c:103: the image brought to TopLeft from `orientation` (the reference's own dispatch to
+    Flop, Flip, Transpose, Transverse and RotateImage by 90, 180 or 270 degrees, which is IntegralRotateImage).
+    Undefined and TopLeft raise MB200_EUNSUPPORTED: the reference returns a clone."""
+    ops = {TopRightOrientation: (GeometryFlop, ()), BottomRightOrientation: (GeometryIntegralRotate, (2,)),
+           BottomLeftOrientation: (GeometryFlip, ()), LeftTopOrientation: (GeometryTranspose, ()),
+           RightTopOrientation: (GeometryIntegralRotate, (1,)), RightBottomOrientation: (GeometryTransverse, ()),
+           LeftBottomOrientation: (GeometryIntegralRotate, (3,))}
+    if orientation not in ops:
+        raise MagickB200Error(_lib.EUNSUPPORTED, "auto-orient: already TopLeft (the reference returns a clone)")
+    return _geometry(image, *ops[orientation])
 
 
 def SampleImage(image: Image, columns: int, rows: int) -> Image:

@@ -479,6 +479,16 @@ int mb200_distort_image_dev(const float *src, size_t width, size_t height, int c
   return launch_distort(src, width, height, channels, dst, plan, options, s);
 }
 
+int mb200_geometry_image_dev(const float *src, size_t width, size_t height, int channels, float *dst,
+                             const mb200_geometry_params *plan, void *stream) {
+  if (!src || !dst || src == dst) return fail(MB200_EINVAL, "geometry: bad arguments");
+  int rc = geometry_check(width, height, channels, plan);
+  cudaStream_t s;
+  if (!rc) rc = prepare(stream, &s);
+  if (rc) return rc;
+  return launch_geometry(src, width, height, channels, dst, plan, s);
+}
+
 int mb200_convolve_image_dev(const float *src, float *dst, size_t width, size_t height, int channels,
                              const mb200_kernel_info *kernel, void *stream) {
   return mb200_morphology_image_dev(src, dst, width, height, channels, MB200_ConvolveMorphology, 1, kernel, 0.0,
@@ -666,6 +676,16 @@ int mb200_distort_image(const float *src, size_t w, size_t h, int ch, float *dst
   if (rc) return rc;
   return with_staging("distort", src, w, h, ch, dst, plan->columns, plan->rows, [&](const float *s, float *d, cudaStream_t st) {
     return mb200_distort_image_dev(s, w, h, ch, d, plan, options, st);
+  });
+}
+
+int mb200_geometry_image(const float *src, size_t w, size_t h, int ch, float *dst, const mb200_geometry_params *plan) {
+  if (!src || !dst) return fail(MB200_EINVAL, "geometry: bad arguments");
+  const int rc = geometry_check(w, h, ch, plan);
+  if (rc) return rc;
+  return with_staging("geometry", src, w, h, ch, dst, plan->columns, plan->rows, ch,
+                      [&](const float *s, float *d, cudaStream_t st) {
+    return mb200_geometry_image_dev(s, w, h, ch, d, plan, st);
   });
 }
 

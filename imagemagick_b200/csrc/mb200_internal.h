@@ -43,6 +43,7 @@ enum LaunchFamily {
   kMorphStream,                                                        // morph_stream.cu
   kMorphDirect,                                                        // morph_direct.cu
   kDistort,                                                            // distort.cu
+  kGeometry,                                                           // geometry.cu
   kLaunchFamilies
 };
 void count_family(LaunchFamily family);
@@ -135,6 +136,12 @@ int distort_check(size_t width, size_t height, int channels, const mb200_distort
                   const mb200_resample_options *options);
 int launch_distort(const float *src, size_t width, size_t height, int channels, float *dst,
                    const mb200_distort_params *plan, const mb200_resample_options *options, void *stream);
+
+// geometry.cu: the orientation and crop operators for a plan of geometry_plan.cpp.  The check runs on the host before
+// anything is touched (MB200_EINVAL: a plan that does not fit the source); the launch is one kernel.
+int geometry_check(size_t width, size_t height, int channels, const mb200_geometry_params *plan);
+int launch_geometry(const float *src, size_t width, size_t height, int channels, float *dst,
+                    const mb200_geometry_params *plan, void *stream);
 
 // ---- resize axis tables (resize_tables.cpp) ---------------------------------
 // One axis of ResizeImage, planned on the host and resident on one device: the reference's contribution lists

@@ -11,7 +11,9 @@
           --wrap=DespeckleImage,--wrap=LocalContrastImage,--wrap=WaveletDenoiseImage,\
           --wrap=ContrastImage,--wrap=ModulateImage,--wrap=GrayscaleImage,--wrap=FunctionImage,\
           --wrap=ContrastStretchImage,--wrap=NormalizeImage,--wrap=LinearStretchImage,--wrap=LevelImage,\
-          --wrap=LevelizeImage,--wrap=MinMaxStretchImage,--wrap=GammaImage
+          --wrap=LevelizeImage,--wrap=MinMaxStretchImage,--wrap=GammaImage,--wrap=DistortImage,--wrap=RotateImage,\
+          --wrap=FlipImage,--wrap=FlopImage,--wrap=TransposeImage,--wrap=TransverseImage,--wrap=IntegralRotateImage,\
+          --wrap=CropImage,--wrap=CropImageToTiles,--wrap=ShaveImage,--wrap=RollImage,--wrap=AutoOrientImage
   and every caller of those exported functions (effect.c:765/1709/1170/4256, morphology.c:4129,
   resize.c:3761, colorspace.c:1751, threshold.c:805/927/2518/1087, effect.c:1308/2013, visual-effects.c:3515,
   enhance.c:1370/3461/2474/1544/4130/3347/2913/3062/2322, histogram.c:927, statistic.c:1064) reaches __wrap_X below.  Each wrapper follows the accelerate
@@ -1574,6 +1576,200 @@ Image *__wrap_RotateImage(const Image *image, const double degrees, ExceptionInf
 {
   TRY(B200AccelerateRotateImage(image, degrees, exception));
   return __real_RotateImage(image, degrees, exception);
+}
+
+/* ---- the orientation and crop operators (transform.c, shear.c) -------------------------------------------------------
+   mb200_geometry_plan gives the output's size and page; the result is CloneImage(image, columns, rows) as the reference
+   clones it, its pixels written by mb200_geometry_image, then the page and type the reference sets.  Calls between these
+   operators inside transform.o (AutoOrientImage -> FlipImage, CropImageToTiles / ShaveImage -> CropImage) and from
+   distort.o's RotateImage to shear.o's IntegralRotateImage are served by the wraps of their callers or cross objects.
+   NULL == declined, with the caller's exception untouched: no device, a layout the library does not take (CMYK,
+   PseudoClass, masks, meta channels), and the plan's declines (a crop outside the canvas or of zero area, a shave of
+   half the image, IntegralRotateImage by 0). */
+static Image *b200_geometry(const Image *image, int op, const long *args)
+{
+  mb200_geometry_params plan;
+  mb200_page page;
+  Image *out = (Image *) NULL;
+  int ch;
+  if (mb200_device_count() <= 0) return (Image *) NULL;
+  ch = b200_layout_masked(image, (unsigned *) NULL);
+  if (ch == 0) return (Image *) NULL;
+  page.width = image->page.width; page.height = image->page.height; page.x = (long) image->page.x;
+  page.y = (long) image->page.y;
+  if (mb200_geometry_plan(op, image->columns, image->rows, &page, args, &plan) != MB200_OK) return (Image *) NULL;
+  {
+    B200_ATTEMPT_BEGIN;
+    const float *p = b200_cache_pixels(image, ch, attempt);
+    if (p != (const float *) NULL) out = new_result(image, plan.columns, plan.rows, attempt);
+    if (out != (Image *) NULL) {
+      Quantum *q = GetAuthenticPixels(out, 0, 0, out->columns, out->rows, attempt);
+      if (q == (Quantum *) NULL || b200_cache_pixels(out, ch, attempt) != (float *) q ||
+          mb200_geometry_image(p, image->columns, image->rows, ch, (float *) q, &plan) != MB200_OK ||
+          SyncAuthenticPixels(out, attempt) == MagickFalse)
+        out = DestroyImage(out);
+    }
+    B200_ATTEMPT_END;
+  }
+  if (out != (Image *) NULL) {
+    out->page.width = plan.page.width; out->page.height = plan.page.height;
+    out->page.x = (ssize_t) plan.page.x; out->page.y = (ssize_t) plan.page.y;
+    out->type = image->type;
+  }
+  return out;
+}
+
+static Image *b200_crop(const Image *image, const RectangleInfo *geometry)
+{
+  const long args[4] = { (long) geometry->width, (long) geometry->height, (long) geometry->x, (long) geometry->y };
+  return b200_geometry(image, MB200_GeometryCrop, args);
+}
+
+/* AutoOrientImage (transform.c:103): the reference's dispatch; Undefined / TopLeft (a clone) decline. */
+static Image *b200_auto_orient(const Image *image, const OrientationType orientation)
+{
+  long rotations = 0;
+  int op;
+  Image *out;
+  switch (orientation) {
+    case TopRightOrientation: op = MB200_GeometryFlop; break;
+    case BottomRightOrientation: op = MB200_GeometryIntegralRotate; rotations = 2; break;   /* RotateImage(180) */
+    case BottomLeftOrientation: op = MB200_GeometryFlip; break;
+    case LeftTopOrientation: op = MB200_GeometryTranspose; break;
+    case RightTopOrientation: op = MB200_GeometryIntegralRotate; rotations = 1; break;     /* RotateImage(90) */
+    case RightBottomOrientation: op = MB200_GeometryTransverse; break;
+    case LeftBottomOrientation: op = MB200_GeometryIntegralRotate; rotations = 3; break;   /* RotateImage(270) */
+    default: return (Image *) NULL;
+  }
+  out = b200_geometry(image, op, &rotations);
+  if (out != (Image *) NULL) out->orientation = TopLeftOrientation;
+  return out;
+}
+
+/* CropImageToTiles (transform.c:791): the geometry parsed with the reference's own ParseGravityGeometry; the single
+   region (with the `!` page fix-up) and the fixed-size WxH tiles as the same loop of served crops.  The `@` tiles and the
+   final clone decline, and so does a tile loop any of whose crops declines. */
+static Image *b200_crop_to_tiles(const Image *image, const char *crop_geometry)
+{
+  RectangleInfo geometry;
+  MagickStatusType flags;
+  ExceptionType severity;
+  Image *list = (Image *) NULL;
+  if (mb200_device_count() <= 0 || b200_layout_masked(image, (unsigned *) NULL) == 0 ||
+      crop_geometry == (const char *) NULL) return (Image *) NULL;
+  {
+    B200_ATTEMPT_BEGIN;
+    flags = ParseGravityGeometry(image, crop_geometry, &geometry, attempt);
+    severity = attempt->severity;
+    B200_ATTEMPT_END;
+  }
+  if (severity != UndefinedException || (flags & AreaValue) != 0) return (Image *) NULL;
+  if ((geometry.width == 0 && geometry.height == 0) || (flags & XValue) != 0 || (flags & YValue) != 0) {
+    list = b200_crop(image, &geometry);
+    if (list != (Image *) NULL && (flags & AspectValue) != 0) {
+      list->page.width = geometry.width;
+      list->page.height = geometry.height;
+      list->page.x -= geometry.x;
+      list->page.y -= geometry.y;
+    }
+    return list;
+  }
+  if (image->columns > geometry.width || image->rows > geometry.height) {
+    RectangleInfo page = image->page;
+    size_t width, height;
+    ssize_t x, y;
+    if (page.width == 0) page.width = image->columns;
+    if (page.height == 0) page.height = image->rows;
+    width = geometry.width == 0 ? page.width : geometry.width;
+    height = geometry.height == 0 ? page.height : geometry.height;
+    for (y = 0; y < (ssize_t) page.height; y += (ssize_t) height)
+      for (x = 0; x < (ssize_t) page.width; x += (ssize_t) width) {
+        Image *next;
+        geometry.width = width; geometry.height = height; geometry.x = x; geometry.y = y;
+        next = b200_crop(image, &geometry);
+        if (next == (Image *) NULL) {
+          if (list != (Image *) NULL) list = DestroyImageList(list);
+          return (Image *) NULL;
+        }
+        AppendImageToList(&list, next);
+      }
+    return list;
+  }
+  return (Image *) NULL;
+}
+
+extern Image *__real_FlipImage(const Image *, ExceptionInfo *);
+extern Image *__real_FlopImage(const Image *, ExceptionInfo *);
+extern Image *__real_TransposeImage(const Image *, ExceptionInfo *);
+extern Image *__real_TransverseImage(const Image *, ExceptionInfo *);
+extern Image *__real_IntegralRotateImage(const Image *, size_t, ExceptionInfo *);
+extern Image *__real_CropImage(const Image *, const RectangleInfo *, ExceptionInfo *);
+extern Image *__real_CropImageToTiles(const Image *, const char *, ExceptionInfo *);
+extern Image *__real_ShaveImage(const Image *, const RectangleInfo *, ExceptionInfo *);
+extern Image *__real_RollImage(const Image *, const ssize_t, const ssize_t, ExceptionInfo *);
+extern Image *__real_AutoOrientImage(const Image *, const OrientationType, ExceptionInfo *);
+
+Image *__wrap_FlipImage(const Image *image, ExceptionInfo *exception)
+{
+  TRY(b200_geometry(image, MB200_GeometryFlip, (const long *) NULL));
+  return __real_FlipImage(image, exception);
+}
+
+Image *__wrap_FlopImage(const Image *image, ExceptionInfo *exception)
+{
+  TRY(b200_geometry(image, MB200_GeometryFlop, (const long *) NULL));
+  return __real_FlopImage(image, exception);
+}
+
+Image *__wrap_TransposeImage(const Image *image, ExceptionInfo *exception)
+{
+  TRY(b200_geometry(image, MB200_GeometryTranspose, (const long *) NULL));
+  return __real_TransposeImage(image, exception);
+}
+
+Image *__wrap_TransverseImage(const Image *image, ExceptionInfo *exception)
+{
+  TRY(b200_geometry(image, MB200_GeometryTransverse, (const long *) NULL));
+  return __real_TransverseImage(image, exception);
+}
+
+Image *__wrap_IntegralRotateImage(const Image *image, size_t rotations, ExceptionInfo *exception)
+{
+  const long r = (long) (rotations % 4);
+  TRY(b200_geometry(image, MB200_GeometryIntegralRotate, &r));
+  return __real_IntegralRotateImage(image, rotations, exception);
+}
+
+Image *__wrap_CropImage(const Image *image, const RectangleInfo *geometry, ExceptionInfo *exception)
+{
+  TRY(b200_crop(image, geometry));
+  return __real_CropImage(image, geometry, exception);
+}
+
+Image *__wrap_CropImageToTiles(const Image *image, const char *crop_geometry, ExceptionInfo *exception)
+{
+  TRY(b200_crop_to_tiles(image, crop_geometry));
+  return __real_CropImageToTiles(image, crop_geometry, exception);
+}
+
+Image *__wrap_ShaveImage(const Image *image, const RectangleInfo *shave_info, ExceptionInfo *exception)
+{
+  const long args[2] = { (long) shave_info->width, (long) shave_info->height };
+  TRY(b200_geometry(image, MB200_GeometryShave, args));
+  return __real_ShaveImage(image, shave_info, exception);
+}
+
+Image *__wrap_RollImage(const Image *image, const ssize_t x_offset, const ssize_t y_offset, ExceptionInfo *exception)
+{
+  const long args[2] = { (long) x_offset, (long) y_offset };
+  TRY(b200_geometry(image, MB200_GeometryRoll, args));
+  return __real_RollImage(image, x_offset, y_offset, exception);
+}
+
+Image *__wrap_AutoOrientImage(const Image *image, const OrientationType orientation, ExceptionInfo *exception)
+{
+  TRY(b200_auto_orient(image, orientation));
+  return __real_AutoOrientImage(image, orientation, exception);
 }
 
 MagickBooleanType __wrap_NormalizeImage(Image *image, ExceptionInfo *exception)

@@ -343,6 +343,37 @@ typedef struct mb200_resample_options {
 /* The cylindrical weight table of SetResampleFilter (resample.c:1246-1300): lut[MB200_RESAMPLE_LUT], *support. */
 MB200_API int mb200_resample_filter_lut(int filter, const mb200_filter_options *options, double *lut, double *support);
 
+/* ---- The orientation and crop operators of MagickCore/transform.c and shear.c: pure data movement ----
+   mb200_geometry_plan runs on the host without a device.  It restates the output geometry and page of
+     CropImage (transform.c:542)       args: width, height, x, y (the RectangleInfo; width / height 0 = the page's)
+     ShaveImage (transform.c:1641)     args: width, height
+     FlipImage, FlopImage (:1194, :1329), TransposeImage, TransverseImage (:2127, :2265)   no args
+     IntegralRotateImage (shear.c:700) args: rotations (taken mod 4 as a size_t, so -1 is 3)
+     RollImage (transform.c:1546)      args: x_offset, y_offset
+   in the reference's arithmetic and order, and the map out(x, y) = in(map(x, y)) the kernel runs.  MB200_EUNSUPPORTED
+   where the reference returns no image of the operation's own (it warns "GeometryDoesNotContainImage": a crop outside
+   the virtual canvas, which it answers with a transparent 1x1 image, a crop of zero area, a shave of half the image or
+   more) and for IntegralRotateImage by 0 (a CloneImage); MB200_EINVAL: an empty image, another op. */
+typedef enum {
+  MB200_GeometryCrop = 0, MB200_GeometryShave = 1, MB200_GeometryFlip = 2, MB200_GeometryFlop = 3,
+  MB200_GeometryTranspose = 4, MB200_GeometryTransverse = 5, MB200_GeometryIntegralRotate = 6, MB200_GeometryRoll = 7
+} mb200_geometry_op;
+/* The dihedral transforms of the map: bit 0 mirrors the source x, bit 1 the source y, bit 2 swaps the axes first. */
+typedef enum {
+  MB200_MapIdentity = 0, MB200_MapFlop = 1, MB200_MapFlip = 2, MB200_MapRotate180 = 3,
+  MB200_MapTranspose = 4, MB200_MapRotate270 = 5, MB200_MapRotate90 = 6, MB200_MapTransverse = 7
+} mb200_geometry_map;
+typedef struct mb200_page { size_t width, height; long x, y; } mb200_page;   /* the image's RectangleInfo page */
+typedef struct mb200_geometry_params {
+  int map;                       /* mb200_geometry_map */
+  size_t columns, rows;          /* the output image */
+  mb200_page page;               /* the output's page */
+  long src_x, src_y;             /* the source rectangle's origin (its size is the output's, swapped by bit 2) */
+  long roll_x, roll_y;           /* RollImage's offsets, in [0, columns) x [0, rows): out(x, y) = in(x - roll_x, ...) */
+} mb200_geometry_params;
+MB200_API int mb200_geometry_plan(int op, size_t columns, size_t rows, const mb200_page *page, const long *args,
+    mb200_geometry_params *plan);
+
 /* --------------------------------------- device-resident operators (HBM) ---- */
 /* src/dst are DEVICE pointers (from mb200_malloc or any CUDA allocation, e.g. a
    torch tensor's data_ptr()); they must not alias unless stated.  `stream` is a
@@ -391,6 +422,12 @@ MB200_API int mb200_morphology_direct_image_dev(const float *src, float *dst, si
    crosses the output (the reference's blend there reads an alpha sum carried along the row). */
 MB200_API int mb200_distort_image_dev(const float *src, size_t width, size_t height, int channels, float *dst,
     const mb200_distort_params *plan, const mb200_resample_options *options, void *stream);
+
+/* The map of a plan from mb200_geometry_plan: dst (plan->columns x plan->rows x channels, 1-5 channels) receives the
+   source samples as 32-bit words, so every bit pattern (NaN payloads, -0, denormals) is kept.  dst must not alias src.
+   MB200_EINVAL, before the device is touched: a map or source rectangle that does not fit the source image. */
+MB200_API int mb200_geometry_image_dev(const float *src, size_t width, size_t height, int channels, float *dst,
+    const mb200_geometry_params *plan, void *stream);
 
 /* ConvolveImage (MagickCore/effect.c:1170) */
 MB200_API int mb200_convolve_image_dev(const float *src, float *dst, size_t width, size_t height,
@@ -651,6 +688,8 @@ MB200_API int mb200_unsharp_mask_image(const float *src, float *dst, size_t widt
     int channels, double radius, double sigma, double gain, double threshold);
 MB200_API int mb200_distort_image(const float *src, size_t width, size_t height, int channels, float *dst,
     const mb200_distort_params *plan, const mb200_resample_options *options);
+MB200_API int mb200_geometry_image(const float *src, size_t width, size_t height, int channels, float *dst,
+    const mb200_geometry_params *plan);
 MB200_API int mb200_sharpen_image(const float *src, float *dst, size_t width, size_t height, int channels,
     double radius, double sigma);
 MB200_API int mb200_edge_image(const float *src, float *dst, size_t width, size_t height, int channels,

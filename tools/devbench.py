@@ -1,5 +1,6 @@
 """Developer micro-benchmark: device-resident timings of the hot-path operators (CUDA events).
-usage: python tools/devbench.py [blur|resize|lab|dilate|erode|gauss|conv2d|stencils|hooks|enhance|layout|level|direct|distort|all]
+usage: python tools/devbench.py [blur|resize|lab|dilate|erode|gauss|conv2d|stencils|hooks|enhance|layout|level|direct|distort|
+                                 geometry|all]
        [size] [ref]   (ref: distort also times the reference's all-core DistortImage / RotateImage, minutes at 8192^2)"""
 import sys
 from pathlib import Path
@@ -290,3 +291,31 @@ if which in ("distort", "all"):
             line += f"  reference all cores {(time.perf_counter() - t0) * 1e3:9.1f} ms (rc {rc})"
         print(line, flush=True)
     del x
+
+if which in ("geometry", "all"):
+    # The orientation and crop operators at size^2 RGBA, device-resident, with the card and its power limit.  Floor:
+    # 16 B/px read + 16 B/px written per output pixel at the 3.35 TB/s H100 SXM data-sheet HBM bandwidth; a plain
+    # device-to-device copy of the same image is timed beside them.
+    import subprocess
+    DATASHEET = 3350.0
+    try:
+        limit = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i",
+                                str(torch.cuda.current_device())], capture_output=True, text=True, timeout=30).stdout.strip()
+    except (OSError, subprocess.SubprocessError):
+        limit = "unknown"
+    print(f"geometry operators on {torch.cuda.get_device_name()} at a power limit of {limit or 'unknown'}", flush=True)
+    src = torch.rand(size, size, 4, device="cuda") * 65535
+    x = im.Image(src)
+    cases = [("copy (torch clone)", lambda: src.clone(), size * size),
+             ("FlipImage", lambda: im.FlipImage(x), size * size),
+             ("FlopImage", lambda: im.FlopImage(x), size * size),
+             ("TransposeImage", lambda: im.TransposeImage(x), size * size),
+             ("IntegralRotateImage 90", lambda: im.IntegralRotateImage(x, 1), size * size),
+             ("CropImage half", lambda: im.CropImage(x, size // 2, size // 2, size // 4, size // 4), (size // 2) ** 2),
+             ("RollImage +1000+777", lambda: im.RollImage(x, 1000, 777), size * size)]
+    for name, fn, npix in cases:
+        ms = timeit(fn, iters=20, warm=3)
+        floor = npix * 32 / DATASHEET / 1e6
+        print(f"{name:26s} {ms:9.3f} ms  {npix * 32 / ms / 1e6:8.1f} GB/s  floor {floor:6.3f} ms = {floor / ms * 100:5.1f}%",
+              flush=True)
+    del x, src
