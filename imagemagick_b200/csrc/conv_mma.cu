@@ -30,9 +30,11 @@
 // evaluated by a scalar DFMA loop over the window's own taps instead (rare: HDRI images with inf / NaN pixels).
 #include "mb200_internal.h"
 #include "conv_common.cuh"
+#include "tma.cuh"
 
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <cstdint>
 
 namespace mb200 {
@@ -363,83 +365,145 @@ __global__ void __launch_bounds__(128, MINB) conv_mma_kernel(const MmaArgs a, co
 // lane ends up with all four sums of pixel line 4 G + t (tile group G) at outputs g and g + 8.
 //
 // Everything else is conv_mma_kernel's scheme at 16-position blocks: a per-warp ring of NKS + 1 blocks (the window and
-// the block being refilled), samples converted and premultiplied once when staged, one non-finite flag per block, loads
-// two blocks ahead of the ring, and the DMMAs of block b, the staging of block b + NKS and the output stage of block
+// the block being refilled), samples converted and premultiplied once when staged, one non-finite flag per block, and the DMMAs of block b, the staging of block b + NKS and the output stage of block
 // b - 1 in one basic block.  Outputs start at multiples of 16 of the image position (the launcher rounds the strip up),
 // so an output's k-grouping, and its bits, do not depend on the strip.
 template <int NKS>
 struct WideTaps { double k[16 * NKS]; };    // window order, zero past the window
 
+// ---- the TMA-fed wide pass on a persistent grid.  Same staging, DMMAs, non-finite flags and output stage as above; what
+// differs is where the source blocks come from and which strips a warp walks.
+//
+// Loads.  A warp's raw source blocks (16 positions x 8 lines of float4 = 2 KB: 8 px x 16 rows in the column pass, 16 px x
+// 8 lines in the row pass) arrive in a per-warp shared-memory ring of kWideStages slots, each filled by one
+// cp.async.bulk.tensor.2d that lane 0 issues, with an mbarrier transaction count per slot.  A slot is refilled as soon
+// as the warp has read it into registers, so kWideStages - 1 blocks (6 KB) stay in flight per warp without holding any
+// registers.  The quarter-warp reads 128 contiguous bytes of a box row: conflict-free LDS.128 without a swizzle.
+// The TMA unit zero-fills outside the image where the reference clamps to the edge, so boxes are issued at clamped
+// coordinates (inside the image whenever the image is at least 16 positions long) and each position is clamped inside
+// its box when it is read: the staged samples are exactly those of min(max(pos, 0), last).
+//
+// Schedule.  The grid is as many CTAs as fit on the device at once (2 per SM); the (band of 8 lines, strip) tiles are
+// split into one contiguous run per warp, band-major, in whole strips: the runs differ by at most one strip (8192^2 at strip 512:
+// 16 or 15 of 16 384 tiles per warp over 1 056 warps, ~3 % of the pass in tail).  Consecutive strips of one band are one
+// segment: the ring carries on across them without a new prologue.  Outputs still start at multiples of 16 of the
+// image position, so the bits depend neither on the strip nor on the split.
+constexpr int kWideStages = 4;
+constexpr unsigned kWideBoxBytes = 2048;
+
 template <int NKS, int AXIS, int EPI>
-__global__ void __launch_bounds__(128, 3) conv_mma_wide_kernel(const MmaArgs a, const WideTaps<NKS> taps) {
+__global__ void __launch_bounds__(128, 2) conv_mma_wide_kernel(const MmaArgs a, const WideTaps<NKS> taps,
+                                                                const __grid_constant__ CUtensorMap tmap) {
   static_assert(EPI == 0 || AXIS == 1, "the fused epilogue belongs to the final column pass");
   constexpr int NB = NKS + 1;                      // ring blocks: the window + the one being refilled
   constexpr int RR = 16 * NB;                      // ring positions along the filter axis
   constexpr int PW = 36;                           // AXIS 1: doubles per ring row: [RG of 8 px | BA of 8 px | pad 4]
   constexpr int PL = 2 * RR + 8;                   // AXIS 0: doubles per image line of a plane (== 8 mod 16)
   constexpr int kWarpDoubles = AXIS == 1 ? RR * PW : 16 * PL;
-  extern __shared__ __align__(16) double ring_all[];
+  constexpr int W = 4, S = kWideStages;            // warps per CTA, raw slots per warp
+  extern __shared__ __align__(128) unsigned char smem_all[];
+  __shared__ __align__(8) unsigned long long bars[W][S];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  double *ring = ring_all + warp * kWarpDoubles;
+  // TMA destinations must be 128-byte aligned: the raw slots of the four warps first, then the double rings
+  unsigned char *smem = smem_all + ((128u - (static_cast<unsigned>(__cvta_generic_to_shared(smem_all)) & 127u)) & 127u);
+  const unsigned raw_s = static_cast<unsigned>(__cvta_generic_to_shared(smem)) + warp * S * kWideBoxBytes;
+  double *ring = reinterpret_cast<double *>(smem + W * S * kWideBoxBytes) + warp * kWarpDoubles;
   const unsigned ring_s = static_cast<unsigned>(__cvta_generic_to_shared(ring));
+  const unsigned bar_s = static_cast<unsigned>(__cvta_generic_to_shared(&bars[warp][0]));
   const int t4 = lane & 3, g8 = lane >> 2;
 
-  int first, nout, limit, par0;
-  if (AXIS == 1) {
-    par0 = (blockIdx.x * 4 + warp) * 8;
-    if (par0 >= a.width) return;                   // (no CTA-wide barrier anywhere: a warp may leave)
-    first = blockIdx.y * a.strip;
-    nout = min(a.strip, a.height - first);
-    limit = a.height - 1;
-  } else {
-    par0 = (blockIdx.y * 4 + warp) * 8;
-    if (par0 >= a.height) return;
-    first = blockIdx.x * a.strip;
-    nout = min(a.strip, a.width - first);
-    limit = a.width - 1;
-  }
-  const int nblocks = (nout + 15) >> 4;
-  const bool mma_l2pf = a.l2pf != 0;
-  const size_t pitch = static_cast<size_t>(a.width) * 16;
+  // ---- this warp's run of tiles
+  const int len = AXIS == 1 ? a.height : a.width;  // extent along the filter axis
+  const int limit = len - 1;
+  const int nstrips = (len + a.strip - 1) / a.strip;
+  const long long ntiles = static_cast<long long>(((AXIS == 1 ? a.width : a.height) + 7) >> 3) * nstrips;
+  const long long nwarps = static_cast<long long>(gridDim.x) * W, gw = static_cast<long long>(blockIdx.x) * W + warp;
+  const long long per = ntiles / nwarps, extra = ntiles % nwarps;
+  const long long t_begin = gw * per + min(gw, extra), t_end = t_begin + per + (gw < extra ? 1 : 0);
+  if (t_begin >= t_end) return;                    // (no CTA-wide barrier anywhere: a warp may leave)
+  struct Seg { long long end; int band, first, nout; };
+  auto segment = [&](long long t) {                // the strips of t's band from t on, up to the end of the run
+    Seg sg;
+    sg.band = static_cast<int>(t / nstrips);
+    const long long band_end = static_cast<long long>(sg.band + 1) * nstrips;
+    sg.end = min(t_end, band_end);
+    sg.first = static_cast<int>(t - static_cast<long long>(sg.band) * nstrips) * a.strip;
+    sg.nout = min(static_cast<int>(sg.end - static_cast<long long>(sg.band) * nstrips) * a.strip, len) - sg.first;
+    return sg;
+  };
+  // box of the 16 source positions from p0: inside the image where it is long enough; clamped positions index into it
+  auto box_start = [&](int p0) { return min(max(p0, 0), max(limit - 15, 0)); };
 
-  // ---- loader: four pixels per lane and block
+  if (lane == 0) {
+#pragma unroll
+    for (int k = 0; k < S; ++k) mbar_init(bar_s + 8 * k, 1);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncwarp();
+
+  // ---- producer: the raw blocks of every segment in the order they are consumed (a segment of nblocks output blocks
+  // reads nblocks + NKS - 1 source blocks), kept S blocks ahead of the consumer
+  Seg pseg = segment(t_begin);
+  int pj = 0;
+  unsigned np = 0, nc = 0;                         // blocks issued / consumed by this warp
+  auto issue_next = [&]() {                        // warp-uniform
+    if (pseg.band < 0) return;
+    const int s0 = box_start(pseg.first - a.off + 16 * pj);
+    if (lane == 0) {
+      const unsigned k = np % S, bar = bar_s + 8 * k;
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // the slot's generic-proxy reads precede the refill
+      mbar_expect_tx(bar, kWideBoxBytes);
+      if (AXIS == 1) tma_load_2d(raw_s + k * kWideBoxBytes, &tmap, pseg.band * 32, s0, bar);
+      else tma_load_2d(raw_s + k * kWideBoxBytes, &tmap, s0 * 4, pseg.band * 8, bar);
+    }
+    ++np;
+    if (++pj == ((pseg.nout + 15) >> 4) + NKS - 1) {
+      pj = 0;
+      if (pseg.end < t_end) pseg = segment(pseg.end);
+      else pseg.band = -1;
+    }
+  };
+#pragma unroll
+  for (int k = 0; k < S; ++k) issue_next();
+
+  // ---- consumer lanes: four pixels per lane and block
   const int lq = lane & 7, lh = lane >> 3;
-  const char *lbase[4];
   int uoff[4];
+  unsigned raw_off[4];                             // byte offset inside a box, without the position along the filter axis
   unsigned st_off[4];                              // ring offset (doubles) of the RG pair inside block slot 0
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
     if (AXIS == 1) {                               // rows lh + 4 i of the block, pixel column lq
-      lbase[i] = static_cast<const char *>(a.src) + static_cast<size_t>(min(par0 + lq, a.width - 1)) * 16;
       uoff[i] = lh + 4 * i;
+      raw_off[i] = static_cast<unsigned>(lq * 16);
       st_off[i] = static_cast<unsigned>(uoff[i] * PW + 2 * lq);
     } else {                                       // image line lh + 4 (i >> 1), positions lq + 8 (i & 1) of the block
       const int line = lh + 4 * (i >> 1);
-      lbase[i] = static_cast<const char *>(a.src) + static_cast<size_t>(min(par0 + line, a.height - 1)) * pitch;
       uoff[i] = lq + 8 * (i & 1);
+      raw_off[i] = static_cast<unsigned>(line * 256);
       st_off[i] = static_cast<unsigned>(line * PL + 2 * uoff[i]);
     }
   }
+  constexpr unsigned kPosBytes = AXIS == 1 ? 128 : 16;           // raw box bytes per position along the filter axis
   constexpr unsigned kBlockStride = AXIS == 1 ? 16 * PW : 32;     // ring doubles per block slot
   constexpr unsigned kBA = AXIS == 1 ? 16 : 8 * PL;               // RG -> BA plane
-  const size_t lstep = AXIS == 1 ? pitch : 16;
-  const int base = first - a.off;                  // source position of ring block 0, element 0
 
   float4 raw[4];
-  auto fetch = [&](int j) {
+  int base = 0;                                    // source position of the segment's ring block 0, element 0
+  auto take = [&](int j) {                         // raw block j of the segment -> registers; refill its slot
+    const unsigned k = nc % S;
+    mbar_wait(bar_s + 8 * k, (nc / S) & 1u);
+    const int p0 = base + 16 * j, s0 = box_start(p0);
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
-      const unsigned pos = static_cast<unsigned>(min(max(base + 16 * j + uoff[i], 0), limit));
-      raw[i] = __ldg(reinterpret_cast<const float4 *>(lbase[i] + static_cast<size_t>(pos) * lstep));
+      const unsigned pos = static_cast<unsigned>(min(max(p0 + uoff[i], 0), limit) - s0);
+      const unsigned addr = raw_s + k * kWideBoxBytes + raw_off[i] + pos * kPosBytes;
+      asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];"
+                   : "=f"(raw[i].x), "=f"(raw[i].y), "=f"(raw[i].z), "=f"(raw[i].w) : "r"(addr) : "memory");
     }
-  };
-  constexpr int kL2Ahead = 4;
-  auto prefetch_l2 = [&](int j) {
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const unsigned pos = static_cast<unsigned>(min(max(base + 16 * j + uoff[i], 0), limit));
-      asm volatile("prefetch.global.L2 [%0];" ::"l"(lbase[i] + static_cast<size_t>(pos) * lstep));
-    }
+    ++nc;
+    __syncwarp();                                  // every lane has read the slot
+    issue_next();
   };
   unsigned badmask = 0;
   auto stage = [&](int slot) {                     // registers -> ring block `slot`; updates the block's flag
@@ -478,193 +542,192 @@ __global__ void __launch_bounds__(128, 3) conv_mma_wide_kernel(const MmaArgs a, 
   constexpr unsigned kTile[4] = {0, kBA, kT2, kT2 + kBA};       // (G, plane) = (0, RG), (0, BA), (1, RG), (1, BA)
   const unsigned lane_px_off = AXIS == 1 ? static_cast<unsigned>(2 * t4) : static_cast<unsigned>(t4 * PL);
 
-  // ---- output stage: the lane holds pixel line 4 G + t4 at outputs g8 and g8 + 8 of a block
-  char *outp;                                      // output of (block, m = g8, G = 0); lags the MMAs by one block
-  if (AXIS == 1) {
-    outp = static_cast<char *>(a.dst) + static_cast<size_t>(first + g8) * pitch + static_cast<size_t>(par0 + t4) * 16;
-  } else {
-    outp = static_cast<char *>(a.dst) + static_cast<size_t>(par0 + t4) * pitch + static_cast<size_t>(first + g8) * 16;
-  }
+  const size_t pitch = static_cast<size_t>(a.width) * 16;
   const size_t ostep = AXIS == 1 ? 16 * pitch : 16 * 16;          // per block
   const size_t gstep = AXIS == 1 ? 4 * 16 : 4 * pitch;            // G 0 -> 1
   const size_t hstep = AXIS == 1 ? 8 * pitch : 8 * 16;            // output g8 -> g8 + 8
-  bool gvalid[2];
-#pragma unroll
-  for (int g = 0; g < 2; ++g) gvalid[g] = (par0 + 4 * g + t4) < (AXIS == 1 ? a.width : a.height);
-  auto output = [&](const double (&acc)[4][4], const float4 (&epi)[2][2], int mrem) {    // mrem: outputs left in the block
-#pragma unroll
-    for (int g = 0; g < 2; ++g)
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const double sr = acc[2 * g][2 * h], sg = acc[2 * g][2 * h + 1], sbv = acc[2 * g + 1][2 * h],
-                     sa = acc[2 * g + 1][2 * h + 1];
-        const double r = fast_reciprocal(clamp_denominator(sa));
-        float4 out = make_float4(static_cast<float>(sr * r), static_cast<float>(sg * r), static_cast<float>(sbv * r),
-                                 static_cast<float>(sa));
-        if (EPI) {
-          out.x = unsharp_point(epi[g][h].x, out.x, a.gain, a.qthreshold);
-          out.y = unsharp_point(epi[g][h].y, out.y, a.gain, a.qthreshold);
-          out.z = unsharp_point(epi[g][h].z, out.z, a.gain, a.qthreshold);
-          out.w = unsharp_point(epi[g][h].w, out.w, a.gain, a.qthreshold);
-        }
-        if (g8 + 8 * h < mrem && gvalid[g]) *reinterpret_cast<float4 *>(outp + g * gstep + h * hstep) = out;
-      }
-  };
-
-  // ---- prologue: the NKS blocks of the first window (all loads in flight together), then the two blocks after it
-  {
-    float4 pre[NKS][4];
-#pragma unroll
-    for (int j = 0; j < NKS; ++j) {
-      fetch(j);
-#pragma unroll
-      for (int i = 0; i < 4; ++i) pre[j][i] = raw[i];
-    }
-#pragma unroll
-    for (int j = 0; j < NKS; ++j) {
-#pragma unroll
-      for (int i = 0; i < 4; ++i) raw[i] = pre[j][i];
-      stage(j);
-    }
-  }
-  float4 ahead[4];                                 // the block after the one in `raw`
-  fetch(NKS + 1);
-#pragma unroll
-  for (int i = 0; i < 4; ++i) ahead[i] = raw[i];
-  fetch(NKS);
-
-  int st_slot = NKS, sb = 0;                       // slot staged in this iteration / first slot of the window
-  double prev[4][4];
-#pragma unroll
-  for (int t = 0; t < 4; ++t)
-#pragma unroll
-    for (int i = 0; i < 4; ++i) prev[t][i] = (i & 1) ? 1.0 : 0.0;
-  float4 epi_prev[2][2], epi_cur[2][2];
-#pragma unroll
-  for (int g = 0; g < 2; ++g)
-#pragma unroll
-    for (int h = 0; h < 2; ++h) epi_prev[g][h] = epi_cur[g][h] = make_float4(0.f, 0.f, 0.f, 0.f);
-  int prev_rem = 0;                                // block -1 does not exist
 
 #pragma unroll 1
-  for (int b = 0; b < nblocks; ++b) {
-    __syncwarp();
-    const int mrem = nout - 16 * b;
-    const unsigned window_bad = badmask & ~(1u << st_slot);     // flags of the slots this block's windows read
-    // Output stage of the previous block and staging of the next one come BEFORE this block's DMMAs in the source, so
-    // that `prev` and the staged registers are dead while the accumulators and B fragments are live (168 registers at
-    // three CTAs per SM); ptxas still interleaves them with the DMMAs, which are in the same basic block.
-    output(prev, epi_prev, prev_rem);
-    if (b > 0) outp += ostep;
-    if (EPI) {                                     // the source pixels of block b: aux at outp's offset (outp is at block b here)
-      const char *epip = reinterpret_cast<const char *>(a.aux) + (outp - static_cast<char *>(a.dst));
-#pragma unroll
-      for (int g = 0; g < 2; ++g)
-#pragma unroll
-        for (int h = 0; h < 2; ++h)
-          if (g8 + 8 * h < mrem && gvalid[g])
-            epi_cur[g][h] = __ldg(reinterpret_cast<const float4 *>(epip + g * gstep + h * hstep));
+  for (long long tile = t_begin; tile < t_end;) {
+    const Seg sg = segment(tile);
+    tile = sg.end;
+    const int par0 = sg.band * 8, first = sg.first, nout = sg.nout;
+    const int nblocks = (nout + 15) >> 4;
+    base = first - a.off;
+
+    // ---- output stage: the lane holds pixel line 4 G + t4 at outputs g8 and g8 + 8 of a block
+    char *outp;                                    // output of (block, m = g8, G = 0); lags the MMAs by one block
+    if (AXIS == 1) {
+      outp = static_cast<char *>(a.dst) + static_cast<size_t>(first + g8) * pitch + static_cast<size_t>(par0 + t4) * 16;
+    } else {
+      outp = static_cast<char *>(a.dst) + static_cast<size_t>(par0 + t4) * pitch + static_cast<size_t>(first + g8) * 16;
     }
-    // next source block -> ring (the slot no window of this iteration reads; the __syncwarp above orders it after the
-    // previous iteration's reads), the one after it -> registers
-    stage(st_slot);
+    bool gvalid[2];
 #pragma unroll
-    for (int i = 0; i < 4; ++i) raw[i] = ahead[i];
-    {
-      float4 keep[4];
-#pragma unroll
-      for (int i = 0; i < 4; ++i) keep[i] = raw[i];
-      fetch(b + NKS + 2);
-      if (mma_l2pf) prefetch_l2(b + NKS + 2 + kL2Ahead);
-#pragma unroll
-      for (int i = 0; i < 4; ++i) { ahead[i] = raw[i]; raw[i] = keep[i]; }
-    }
-    double acc[4][4];
-#pragma unroll
-    for (int t = 0; t < 4; ++t)
-#pragma unroll
-      for (int i = 0; i < 4; ++i) acc[t][i] = 0.0;
-    {
-      // B fragments, one (k-step, tile) at a time, loaded one DMMA ahead (a DMMA.16x8x16 occupies the pipe for ~64
-      // cycles, longer than an LDS takes)
-      unsigned ua[NKS];
-#pragma unroll
-      for (int s = 0; s < NKS; ++s) {
-        const int blk = sb + s >= NB ? sb + s - NB : sb + s;
-        ua[s] = ring_s + (frag_off + static_cast<unsigned>(blk) * kBlockStride) * 8u;
-      }
-      auto lds4 = [&](double (&bv)[4], int q) {
-        const unsigned addr = ua[q >> 2] + kTile[q & 3] * 8;          // (q is unrolled: the offsets fold into the LDS)
-#pragma unroll
-        for (int i = 0; i < 4; ++i)
-          asm volatile("ld.shared.f64 %0, [%1];" : "=d"(bv[i]) : "r"(addr + 4 * i * kUStride * 8));
-      };
-      double bq[2][4];
-      lds4(bq[0], 0);
-#pragma unroll
-      for (int q = 0; q < 4 * NKS; ++q) {
-        if (q + 1 < 4 * NKS) lds4(bq[(q + 1) & 1], q + 1);
-        const double *av = atap + 4 * (q >> 2);     // element i: av[(i >> 1) + 2 - 2 (i & 1)]
-        double (&d)[4] = acc[q & 3];
-        const double (&bv)[4] = bq[q & 1];
-        asm volatile("mma.sync.aligned.m16n8k16.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7,%8,%9,%10,%11}, "
-                     "{%12,%13,%14,%15}, {%0,%1,%2,%3};"
-                     : "+d"(d[0]), "+d"(d[1]), "+d"(d[2]), "+d"(d[3])
-                     : "d"(av[2]), "d"(av[0]), "d"(av[3]), "d"(av[1]), "d"(av[4]), "d"(av[2]), "d"(av[5]), "d"(av[3]),
-                       "d"(bv[0]), "d"(bv[1]), "d"(bv[2]), "d"(bv[3]));
-      }
-    }
-    if (window_bad != 0) {
-      // a window of this block holds a non-finite sample: the window's own taps only, in scalar FMAs
+    for (int g = 0; g < 2; ++g) gvalid[g] = (par0 + 4 * g + t4) < (AXIS == 1 ? a.width : a.height);
+    auto output = [&](const double (&acc)[4][4], const float4 (&epi)[2][2], int mrem) {    // mrem: outputs left in the block
 #pragma unroll
       for (int g = 0; g < 2; ++g)
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
-          double s0 = 0.0, s1 = 0.0, s2 = 0.0, s3 = 0.0;
-          int u = 16 * sb + g8 + 8 * h;
-          if (u >= RR) u -= RR;
-          for (int t = 0; t < a.ntaps; ++t) {
-            const double *p = ring + static_cast<unsigned>(u) * kUStride + lane_px_off + g * kT2;
-            const double2 rg = *reinterpret_cast<const double2 *>(p);
-            const double2 ba = *reinterpret_cast<const double2 *>(p + kBA);
-            const double k = taps.k[t];
-            s0 = fma(k, rg.x, s0); s1 = fma(k, rg.y, s1); s2 = fma(k, ba.x, s2); s3 = fma(k, ba.y, s3);
-            if (++u == RR) u = 0;
+          const double sr = acc[2 * g][2 * h], sg = acc[2 * g][2 * h + 1], sbv = acc[2 * g + 1][2 * h],
+                       sa = acc[2 * g + 1][2 * h + 1];
+          const double r = fast_reciprocal(clamp_denominator(sa));
+          float4 out = make_float4(static_cast<float>(sr * r), static_cast<float>(sg * r), static_cast<float>(sbv * r),
+                                   static_cast<float>(sa));
+          if (EPI) {
+            out.x = unsharp_point(epi[g][h].x, out.x, a.gain, a.qthreshold);
+            out.y = unsharp_point(epi[g][h].y, out.y, a.gain, a.qthreshold);
+            out.z = unsharp_point(epi[g][h].z, out.z, a.gain, a.qthreshold);
+            out.w = unsharp_point(epi[g][h].w, out.w, a.gain, a.qthreshold);
           }
-          acc[2 * g][2 * h] = s0; acc[2 * g][2 * h + 1] = s1; acc[2 * g + 1][2 * h] = s2; acc[2 * g + 1][2 * h + 1] = s3;
+          if (g8 + 8 * h < mrem && gvalid[g]) *reinterpret_cast<float4 *>(outp + g * gstep + h * hstep) = out;
         }
+    };
+
+    // ---- prologue: the NKS blocks of the first window, then the block after it into registers
+    badmask = 0;
+#pragma unroll
+    for (int j = 0; j < NKS; ++j) {
+      take(j);
+      stage(j);
     }
+    if (nblocks > 1) take(NKS);
+
+    int st_slot = NKS, sb = 0;                     // slot staged in this iteration / first slot of the window
+    double prev[4][4];
 #pragma unroll
     for (int t = 0; t < 4; ++t)
 #pragma unroll
-      for (int i = 0; i < 4; ++i) prev[t][i] = acc[t][i];
-    if (EPI) {
+      for (int i = 0; i < 4; ++i) prev[t][i] = (i & 1) ? 1.0 : 0.0;
+    float4 epi_prev[2][2], epi_cur[2][2];
 #pragma unroll
-      for (int g = 0; g < 2; ++g)
+    for (int g = 0; g < 2; ++g)
 #pragma unroll
-        for (int h = 0; h < 2; ++h) epi_prev[g][h] = epi_cur[g][h];
+      for (int h = 0; h < 2; ++h) epi_prev[g][h] = epi_cur[g][h] = make_float4(0.f, 0.f, 0.f, 0.f);
+    int prev_rem = 0;                              // block -1 does not exist
+
+#pragma unroll 1
+    for (int b = 0; b < nblocks; ++b) {
+      __syncwarp();
+      const int mrem = nout - 16 * b;
+      const unsigned window_bad = badmask & ~(1u << st_slot);     // flags of the slots this block's windows read
+      // Output stage of the previous block and staging of the next one come BEFORE this block's DMMAs in the source, so
+      // that `prev` and the staged registers are dead while the accumulators are live; ptxas interleaves them with the
+      // DMMAs, which are in the same basic block.
+      output(prev, epi_prev, prev_rem);
+      if (b > 0) outp += ostep;
+      if (EPI) {                                   // the source pixels of block b: aux at outp's offset (outp is at block b here)
+        const char *epip = reinterpret_cast<const char *>(a.aux) + (outp - static_cast<char *>(a.dst));
+#pragma unroll
+        for (int g = 0; g < 2; ++g)
+#pragma unroll
+          for (int h = 0; h < 2; ++h)
+            if (g8 + 8 * h < mrem && gvalid[g])
+              epi_cur[g][h] = __ldg(reinterpret_cast<const float4 *>(epip + g * gstep + h * hstep));
+      }
+      // next source block -> ring (the slot no window of this iteration reads; the __syncwarp above orders it after the
+      // previous iteration's reads)
+      if (b + 1 < nblocks) stage(st_slot);
+      double acc[4][4];
+#pragma unroll
+      for (int t = 0; t < 4; ++t)
+#pragma unroll
+        for (int i = 0; i < 4; ++i) acc[t][i] = 0.0;
+      {
+        // B fragments, one (k-step, tile) at a time, loaded one DMMA ahead (a DMMA.16x8x16 occupies the pipe for ~64
+        // cycles, longer than an LDS takes)
+        unsigned ua[NKS];
+#pragma unroll
+        for (int s = 0; s < NKS; ++s) {
+          const int blk = sb + s >= NB ? sb + s - NB : sb + s;
+          ua[s] = ring_s + (frag_off + static_cast<unsigned>(blk) * kBlockStride) * 8u;
+        }
+        auto lds4 = [&](double (&bv)[4], int q) {
+          const unsigned addr = ua[q >> 2] + kTile[q & 3] * 8;        // (q is unrolled: the offsets fold into the LDS)
+#pragma unroll
+          for (int i = 0; i < 4; ++i)
+            asm volatile("ld.shared.f64 %0, [%1];" : "=d"(bv[i]) : "r"(addr + 4 * i * kUStride * 8));
+        };
+        double bq[2][4];
+        lds4(bq[0], 0);
+#pragma unroll
+        for (int q = 0; q < 4 * NKS; ++q) {
+          if (q + 1 < 4 * NKS) lds4(bq[(q + 1) & 1], q + 1);
+          const double *av = atap + 4 * (q >> 2);   // element i: av[(i >> 1) + 2 - 2 (i & 1)]
+          double (&d)[4] = acc[q & 3];
+          const double (&bv)[4] = bq[q & 1];
+          asm volatile("mma.sync.aligned.m16n8k16.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7,%8,%9,%10,%11}, "
+                       "{%12,%13,%14,%15}, {%0,%1,%2,%3};"
+                       : "+d"(d[0]), "+d"(d[1]), "+d"(d[2]), "+d"(d[3])
+                       : "d"(av[2]), "d"(av[0]), "d"(av[3]), "d"(av[1]), "d"(av[4]), "d"(av[2]), "d"(av[5]), "d"(av[3]),
+                         "d"(bv[0]), "d"(bv[1]), "d"(bv[2]), "d"(bv[3]));
+        }
+      }
+      // the source block staged in the next iteration -> registers
+      if (b + 2 < nblocks) take(b + NKS + 1);
+      if (window_bad != 0) {
+        // a window of this block holds a non-finite sample: the window's own taps only, in scalar FMAs
+#pragma unroll
+        for (int g = 0; g < 2; ++g)
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            double s0 = 0.0, s1 = 0.0, s2 = 0.0, s3 = 0.0;
+            int u = 16 * sb + g8 + 8 * h;
+            if (u >= RR) u -= RR;
+            for (int t = 0; t < a.ntaps; ++t) {
+              const double *p = ring + static_cast<unsigned>(u) * kUStride + lane_px_off + g * kT2;
+              const double2 rg = *reinterpret_cast<const double2 *>(p);
+              const double2 ba = *reinterpret_cast<const double2 *>(p + kBA);
+              const double k = taps.k[t];
+              s0 = fma(k, rg.x, s0); s1 = fma(k, rg.y, s1); s2 = fma(k, ba.x, s2); s3 = fma(k, ba.y, s3);
+              if (++u == RR) u = 0;
+            }
+            acc[2 * g][2 * h] = s0; acc[2 * g][2 * h + 1] = s1; acc[2 * g + 1][2 * h] = s2; acc[2 * g + 1][2 * h + 1] = s3;
+          }
+      }
+#pragma unroll
+      for (int t = 0; t < 4; ++t)
+#pragma unroll
+        for (int i = 0; i < 4; ++i) prev[t][i] = acc[t][i];
+      if (EPI) {
+#pragma unroll
+        for (int g = 0; g < 2; ++g)
+#pragma unroll
+          for (int h = 0; h < 2; ++h) epi_prev[g][h] = epi_cur[g][h];
+      }
+      prev_rem = mrem;
+      st_slot = st_slot + 1 == NB ? 0 : st_slot + 1;
+      if (++sb == NB) sb = 0;
     }
-    prev_rem = mrem;
-    st_slot = st_slot + 1 == NB ? 0 : st_slot + 1;
-    if (++sb == NB) sb = 0;
+    output(prev, epi_prev, prev_rem);
   }
-  output(prev, epi_prev, prev_rem);
 }
 
 template <int NKS, int AXIS, int EPI>
 int launch_wide(const MmaArgs &a, const double *taps_host, cudaStream_t stream) {
   constexpr int RR = 16 * (NKS + 1);
   constexpr int kWarpDoubles = AXIS == 1 ? RR * 36 : 16 * (2 * RR + 8);
-  constexpr size_t smem = 4 * kWarpDoubles * sizeof(double);
+  constexpr size_t smem = 4 * (kWarpDoubles * sizeof(double) + kWideStages * kWideBoxBytes) + 128;
   WideTaps<NKS> taps;
   for (int i = 0; i < 16 * NKS; ++i) taps.k[i] = i < a.ntaps ? taps_host[i] : 0.0;
-  dim3 grid;
-  if (AXIS == 1) grid = dim3((a.width + 31) / 32, (a.height + a.strip - 1) / a.strip);
-  else grid = dim3((a.width + a.strip - 1) / a.strip, (a.height + 31) / 32);
-  if (grid.y > 65535) return MB200_EUNSUPPORTED;
+  // 2 CTAs per SM: the register budget of __launch_bounds__(128, 2), and the rings plus the 1 KB the SM reserves per CTA
+  constexpr int kCtasPerSm = 2;
+  static_assert(kCtasPerSm * (smem + 1024) <= 228 * 1024, "two CTAs' rings must fit in an SM's shared memory");
+  // Column pass: 128-byte box rows, and the neighbouring band's 128 bytes belong to another warp at another point of its
+  // run, so the L2 fetches what a box reads and no more.
+  CUtensorMap tmap;
+  if (!make_rgba_tensor_map(static_cast<const float *>(a.src), a.width, a.height, AXIS == 1 ? 32 : 64, AXIS == 1 ? 16 : 8,
+                            CU_TENSOR_MAP_SWIZZLE_NONE,
+                            AXIS == 1 ? CU_TENSOR_MAP_L2_PROMOTION_L2_128B : CU_TENSOR_MAP_L2_PROMOTION_L2_256B, &tmap))
+    return MB200_EUNSUPPORTED;                     // no tensor-map encoder in the driver: the caller's DFMA kernels
   auto kernel = conv_mma_wide_kernel<NKS, AXIS, EPI>;
-  if (smem > 48 * 1024) cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
-  kernel<<<grid, 128, smem, stream>>>(a, taps);
+  // per device attribute: set on every launch (a few microseconds)
+  cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
+  const long long lines = AXIS == 1 ? a.width : a.height, len = AXIS == 1 ? a.height : a.width;
+  const long long tiles = (lines + 7) / 8 * ((len + a.strip - 1) / a.strip);
+  const int grid = static_cast<int>(std::min<long long>(static_cast<long long>(kCtasPerSm) * sm_count(), (tiles + 3) / 4));
+  kernel<<<grid, 128, smem, stream>>>(a, taps, tmap);
   count_launch();
   count_family(kConvMma);
   count_family(kConvMmaWide);

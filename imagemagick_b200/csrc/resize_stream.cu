@@ -30,8 +30,8 @@
 // short low-binade runs) are produced by the generic gather kernels of resize.cu.
 #include "mb200_internal.h"
 
-#include <cuda.h>                 // CUtensorMap (types only: the encoder is fetched through cudaGetDriverEntryPoint)
-#include <cudaTypedefs.h>
+#include "tma.cuh"
+
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -328,28 +328,6 @@ __global__ void __launch_bounds__(128, MINB) resize_h_stream_kernel(const Stream
 // (a third of the shared-memory wavefronts of the cp.async ring's writes conflict).
 // Rows / pixels outside the image are zero-filled by the TMA unit; the streamed runs never read them into a stored
 // output (clipped windows are border outputs, gathered by the extra CTAs).
-__device__ __forceinline__ void mbar_init(unsigned bar, unsigned count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(unsigned bar, unsigned bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(unsigned bar, unsigned parity) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "MB200_WAIT:\n"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
-      "@p bra MB200_DONE;\n"
-      "bra MB200_WAIT;\n"
-      "MB200_DONE:\n"
-      "}\n" ::"r"(bar), "r"(parity) : "memory");
-}
-__device__ __forceinline__ void tma_load_2d(unsigned dst, const CUtensorMap *map, int c0, int c1, unsigned bar) {
-  asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
-               ::"r"(dst), "l"(map), "r"(c0), "r"(c1), "r"(bar) : "memory");
-}
-
 template <int S, int N, int NSLOT, int MINB, int BOXES = 2>
 __global__ void __launch_bounds__(128, MINB) resize_h_tma_kernel(const StreamArgs a, const __grid_constant__ CUtensorMap tmap) {
   using T = Rot<S, N>;
@@ -439,26 +417,6 @@ __global__ void __launch_bounds__(128, MINB) resize_h_tma_kernel(const StreamArg
       }
     }
   }
-}
-
-// Tensor map of an RGBA float image as a 2-D array of floats (4 * width x height), box = 32 floats x 32 rows, 128-byte
-// swizzle.  The encoder is a driver entry point; the library links the runtime only, so it is fetched by name.
-bool make_row_tensor_map(const float *src, int width, int height, CUtensorMap *map) {
-  static PFN_cuTensorMapEncodeTiled encode = [] {
-    void *fn = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &q) != cudaSuccess ||
-        q != cudaDriverEntryPointSuccess)
-      fn = nullptr;
-    return reinterpret_cast<PFN_cuTensorMapEncodeTiled>(fn);
-  }();
-  if (encode == nullptr) return false;
-  const cuuint64_t dims[2] = {static_cast<cuuint64_t>(width) * 4, static_cast<cuuint64_t>(height)};
-  const cuuint64_t strides[1] = {static_cast<cuuint64_t>(width) * 16};
-  const cuuint32_t box[2] = {32, 32}, estr[2] = {1, 1};
-  return encode(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float *>(src), dims, strides, box, estr,
-                CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
 // ------------------------------------------------------------------------------------------ fused V + H
@@ -742,7 +700,8 @@ int launch_sn(StreamArgs a, int axis, cudaStream_t s) {
   LaunchFamily family = kResizeHStream;
   CUtensorMap tmap;
   if (axis == 0 && tma != 0 && (reinterpret_cast<uintptr_t>(a.src) & 15) == 0 &&
-      make_row_tensor_map(a.src, a.width, a.height, &tmap)) {
+      make_rgba_tensor_map(a.src, a.width, a.height, 32, 32, CU_TENSOR_MAP_SWIZZLE_128B,
+                           CU_TENSOR_MAP_L2_PROMOTION_L2_256B, &tmap)) {
     // TMA-staged ring: 3 slots x 8 KB per warp, 2 CTAs / SM (tma == 2: 2 slots, 3 CTAs / SM)
     family = kResizeHTma;
     if (tma == 2) {
