@@ -95,7 +95,9 @@ struct Rot {
 };
 
 // one source sample into the live accumulators; m = step within the rotation period (static).
-// Slot q holds the output whose window started at step S*q of this (or the previous) period.
+// Slot q holds the output whose window started at step S*q of this (or the previous) period.  A window's first tap
+// starts its sum from +0 as the reference's pixel = 0.0 does (resize.c:3493): fma(w, q, +0) is w*q except that a -0
+// product becomes +0, so a window of -0 products gives +0, not -0.  Same DFMA pipe as the DMUL it replaces.
 template <int S, int N>
 __device__ __forceinline__ void feed(double (&acc)[Rot<S, N>::R][4], const double (&W)[N], const float4 v, int m) {
   constexpr int R = Rot<S, N>::R, P = Rot<S, N>::P;
@@ -105,7 +107,10 @@ __device__ __forceinline__ void feed(double (&acc)[Rot<S, N>::R][4], const doubl
   for (int q = 0; q < R; ++q) {
     const int j = (m - S * q + 2 * P) % P;        // tap index of this sample in slot q's window
     if (j == 0) {
-      acc[q][0] = W[0] * q0; acc[q][1] = W[0] * q1; acc[q][2] = W[0] * q2; acc[q][3] = W[0] * a;
+      acc[q][0] = fma(W[0], q0, 0.0);
+      acc[q][1] = fma(W[0], q1, 0.0);
+      acc[q][2] = fma(W[0], q2, 0.0);
+      acc[q][3] = fma(W[0], a, 0.0);
     } else if (j < N) {
       acc[q][0] = fma(W[j], q0, acc[q][0]);
       acc[q][1] = fma(W[j], q1, acc[q][1]);

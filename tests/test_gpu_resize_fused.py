@@ -7,6 +7,7 @@ import numpy as np
 import pytest
 
 import util
+from resample_edge_cases import SERVED          # (filter, ratio) -> (stride, taps) of the streamed runs
 from util import P, make_image, oracle
 
 pytestmark = pytest.mark.gpu
@@ -14,9 +15,6 @@ pytestmark = pytest.mark.gpu
 im = pytest.importorskip("imagemagick_b200")
 
 FAMILIES = ("resize_fused_launches", "resize_v_stream_launches", "resize_h_tma_launches", "resize_h_stream_launches")
-# (filter, ratio) -> the (stride, taps) of the streamed runs: every pair the streaming kernels serve
-SERVED = {(22, 2): (2, 12), (24, 2): (2, 8), (12, 2): (2, 8), (3, 2): (2, 4), (22, 3): (3, 19), (22, 4): (4, 24),
-          (24, 4): (4, 16)}
 
 
 def _dev(a):

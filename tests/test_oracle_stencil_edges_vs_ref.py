@@ -26,38 +26,39 @@ import util
 from util import P, ROOT, digest
 
 DIGESTS = ROOT / "tests" / "golden" / "stencil_edge_digests.json"
-_stored = None
-_recorded = {}
+_stored = {}                    # digest file -> its contents
+_recorded = {}                  # digest file -> {(test, case): result}
 
 
 def _save_recorded():
-    data = json.loads(DIGESTS.read_text()) if DIGESTS.exists() else {}
-    for (test, case), value in _recorded.items():
-        data.setdefault(test, {})[case] = value
-    DIGESTS.write_text("{\n" + ",\n".join(json.dumps(t) + ": " + json.dumps(c, separators=(",", ":"))
-                                           for t, c in sorted(data.items())) + "\n}\n")
+    for path, recorded in _recorded.items():
+        data = json.loads(path.read_text()) if path.exists() else {}
+        for (test, case), value in recorded.items():
+            data.setdefault(test, {})[case] = value
+        path.write_text("{\n" + ",\n".join(json.dumps(t) + ": " + json.dumps(c, separators=(",", ":"))
+                                            for t, c in sorted(data.items())) + "\n}\n")
 
 
 def _signs(a):
     return digest((a == 0) & np.signbit(a))
 
 
-def reference(case, run):
-    """"<digest>/<zero-sign digest>" of what the reference computed for `case` of the running test.  With
-    MB200_RECORD_REFERENCE=1 and oracle/_ref built, run() computes it with the reference and it is recorded when the
-    process exits."""
-    global _stored
+def reference(case, run, digests=DIGESTS):
+    """"<digest>/<zero-sign digest>" of what the reference computed for `case` of the running test, stored in the file
+    `digests`.  With MB200_RECORD_REFERENCE=1 and oracle/_ref built, run() computes it with the reference and it is
+    recorded when the process exits."""
     test = os.environ.get("PYTEST_CURRENT_TEST", "").rsplit(" (", 1)[0].split("::", 1)
     test = test[0].rsplit("/", 1)[-1] + "::" + test[-1]
     if os.environ.get("MB200_RECORD_REFERENCE") == "1" and util.have_ref():
         if not _recorded:
             atexit.register(_save_recorded)
         out = run()
-        _recorded[test, case] = f"{digest(out)}/{_signs(out)}"
-        return _recorded[test, case]
-    if _stored is None:
-        _stored = json.loads(DIGESTS.read_text())
-    stored = _stored.get(test, {})
+        recorded = _recorded.setdefault(digests, {})
+        recorded[test, case] = f"{digest(out)}/{_signs(out)}"
+        return recorded[test, case]
+    if digests not in _stored:
+        _stored[digests] = json.loads(digests.read_text())
+    stored = _stored[digests].get(test, {})
     assert case in stored, f"no stored reference result for {test} / {case}"
     return stored[case]
 
