@@ -167,6 +167,14 @@ PROTOTYPES = {
     "mb200_black_threshold_image": (_i, [_vp, _sz, _sz, _i, _i, C.c_char_p]),
     "mb200_white_threshold_image": (_i, [_vp, _sz, _sz, _i, _i, C.c_char_p]),
     "mb200_clamp_image": (_i, [_vp, _sz, _sz, _i]),
+    "mb200_adaptive_threshold_image_dev": (_i, [_vp, _vp, _sz, _sz, _i, _sz, _sz, _d, C.c_uint, _vp]),
+    "mb200_auto_threshold_image_dev": (_i, [_vp, _sz, _sz, _i, _i, C.POINTER(_d), _vp]),
+    "mb200_range_threshold_image_dev": (_i, [_vp, _sz, _sz, _i, _d, _d, _d, _d, _i, C.c_uint, _vp]),
+    "mb200_perceptible_image_dev": (_i, [_vp, _sz, _sz, _i, _d, C.c_uint, _vp]),
+    "mb200_adaptive_threshold_image": (_i, [_vp, _vp, _sz, _sz, _i, _sz, _sz, _d, C.c_uint]),
+    "mb200_auto_threshold_image": (_i, [_vp, _sz, _sz, _i, _i, C.POINTER(_d)]),
+    "mb200_range_threshold_image": (_i, [_vp, _sz, _sz, _i, _d, _d, _d, _d, _i, C.c_uint]),
+    "mb200_perceptible_image": (_i, [_vp, _sz, _sz, _i, _d, C.c_uint]),
     "mb200_contrast_image_dev": (_i, [_vp, _sz, _sz, _i, _i, _vp]),
     "mb200_modulate_image_dev": (_i, [_vp, _sz, _sz, _i, _d, _d, _d, _i, _i, _vp]),
     "mb200_grayscale_image_dev": (_i, [_vp, _sz, _sz, _i, _i, _i, _vp]),

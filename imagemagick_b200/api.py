@@ -16,6 +16,7 @@ include/magick_b200.h:
     ResizeImage, SampleImage, ScaleImage, ThumbnailImage (pixel)    resize.c:3761/3907/4106/4591
     TransformImageColorspace                                        colorspace.c:1751
     BilevelImage, BlackThresholdImage, WhiteThresholdImage, ClampImage  threshold.c:805/927/2518/1087
+    AdaptiveThresholdImage, AutoThresholdImage, RangeThresholdImage, PerceptibleImage  threshold.c:182/660/2377/2092
     ContrastImage, ModulateImage, GrayscaleImage                    enhance.c:1370/3461/2474
     FunctionImage                                                   statistic.c:1064
     LevelImage, LevelizeImage, GammaImage                           enhance.c:2913/3062/2322
@@ -83,6 +84,9 @@ _LAYOUT_SPACES = {GRAYColorspace, LinearGRAYColorspace, CMYKColorspace}
 (UndefinedPixelIntensityMethod, AveragePixelIntensityMethod, BrightnessPixelIntensityMethod, LightnessPixelIntensityMethod,
  MSPixelIntensityMethod, Rec601LumaPixelIntensityMethod, Rec601LuminancePixelIntensityMethod, Rec709LumaPixelIntensityMethod,
  Rec709LuminancePixelIntensityMethod, RMSPixelIntensityMethod) = range(10)
+
+# MagickCore/threshold.h AutoThresholdMethod
+UndefinedThresholdMethod, KapurThresholdMethod, OTSUThresholdMethod, TriangleThresholdMethod = range(4)
 
 # MagickCore/statistic.h:130-137
 UndefinedFunction, ArcsinFunction, ArctanFunction, PolynomialFunction, SinusoidFunction = range(5)
@@ -755,6 +759,49 @@ def WhiteThresholdImage(image: Image, thresholds: str) -> bool:
 def ClampImage(image: Image) -> bool:
     """MagickCore/threshold.c:1087 -- in place."""
     return _in_place(image, "mb200_clamp_image_dev", "mb200_clamp_image")
+
+
+def _update_mask(image: Image, channels: Optional[int]) -> int:
+    """The Update channels (bit c = channel c) of a `channels` selection; None = all, alpha included."""
+    return (1 << image.channels) - 1 if channels is None else int(channels) & ((1 << image.channels) - 1)
+
+
+def AdaptiveThresholdImage(image: Image, width: int, height: int, bias: float, channels: Optional[int] = None) -> Image:
+    """MagickCore/threshold.c:182 -- a new image: every Update channel := centre <= mean of the width x height window
+    + bias ? 0 : QuantumRange (`bias` in quantum units); the other channels of a `channels` selection are copied."""
+    return _same_size_op(image, "mb200_adaptive_threshold_image_dev", "mb200_adaptive_threshold_image", int(width),
+                         int(height), float(bias), _update_mask(image, channels))
+
+
+def AutoThresholdImage(image: Image, method: int) -> float:
+    """MagickCore/threshold.c:660 -- in place; returns the threshold in percent (the "auto-threshold:threshold" property
+    is its "%g%%")."""
+    _check_intensity(image, "AutoThresholdImage")
+    threshold = C.c_double(0.0)
+    _in_place(image, "mb200_auto_threshold_image_dev", "mb200_auto_threshold_image", int(method), C.byref(threshold))
+    return float(threshold.value)
+
+
+def RangeThresholdImage(image: Image, low_black: float, low_white: float, high_white: float, high_black: float,
+                        channels: Optional[int] = None) -> bool:
+    """MagickCore/threshold.c:2377 -- in place; a gray image is first transformed to sRGB, as the reference does.
+    Without `channels` every channel is thresholded on the pixel's intensity, with them each selected channel on its
+    own sample."""
+    if image.channels <= 2 or image.colorspace in (GRAYColorspace, LinearGRAYColorspace):
+        if image.colorspace not in (GRAYColorspace, LinearGRAYColorspace):
+            image.colorspace = GRAYColorspace              # a gray (+ alpha) pixel cache
+        TransformImageColorspace(image, sRGBColorspace)
+    _check_intensity(image, "RangeThresholdImage")
+    return _in_place(image, "mb200_range_threshold_image_dev", "mb200_range_threshold_image", float(low_black),
+                     float(low_white), float(high_white), float(high_black), 0 if channels is None else 1,
+                     _update_mask(image, channels))
+
+
+def PerceptibleImage(image: Image, epsilon: float, channels: Optional[int] = None) -> bool:
+    """MagickCore/threshold.c:2092 -- in place: samples of the Update channels closer to 0 than epsilon become
+    +-epsilon."""
+    return _in_place(image, "mb200_perceptible_image_dev", "mb200_perceptible_image", float(epsilon),
+                     _update_mask(image, channels))
 
 
 def ContrastImage(image: Image, sharpen: bool) -> bool:

@@ -837,6 +837,127 @@ int mb200_clamp_image(float *buf, size_t w, size_t h, int ch) {
 
 }  // extern "C"
 
+// ---- AdaptiveThresholdImage (threshold.cu), AutoThresholdImage, RangeThresholdImage, PerceptibleImage -----------------
+namespace {
+
+unsigned update_bits(int channels, unsigned update_mask) { return update_mask & ((1u << channels) - 1u); }
+
+int check_adaptive_window(size_t window_width, size_t window_height) {
+  if (window_width > MB200_ADAPTIVE_THRESHOLD_MAX_WINDOW || window_height > MB200_ADAPTIVE_THRESHOLD_MAX_WINDOW)
+    return fail(MB200_EUNSUPPORTED, "adaptive threshold: window %zux%zu is larger than %d", window_width, window_height,
+                MB200_ADAPTIVE_THRESHOLD_MAX_WINDOW);
+  return MB200_OK;
+}
+
+// AutoThresholdImage counts 32-bit histogram bins (checked before anything is staged)
+int check_auto_threshold(size_t w, size_t h, int method, const double *threshold_percent) {
+  if (!threshold_percent || method < MB200_UndefinedThresholdMethod || method > MB200_TriangleThresholdMethod)
+    return fail(MB200_EINVAL, "auto threshold: bad arguments");
+  if (w != 0 && h > (((static_cast<size_t>(1) << 32) - 1) / w))
+    return fail(MB200_EUNSUPPORTED, "auto threshold: images of 2^32 pixels or more are not supported");
+  return MB200_OK;
+}
+
+// PerceptibleReciprocal (gem-private.h)
+double perceptible_reciprocal(double x) {
+  const double sign = x < 0.0 ? -1.0 : 1.0;
+  return (sign * x) >= 1.0e-12 ? 1.0 / x : sign / 1.0e-12;
+}
+
+int check_range_threshold(int channels) {
+  if (channels < 3) return fail(MB200_EUNSUPPORTED, "range threshold: gray images are transformed to sRGB first (threshold.c:2407)");
+  return MB200_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int mb200_adaptive_threshold_image_dev(const float *src, float *dst, size_t width, size_t height, int channels,
+                                       size_t window_width, size_t window_height, double bias, unsigned update_mask,
+                                       void *stream) {
+  cudaStream_t s;
+  int rc = prepare_dev(src && dst && valid_image(width, height, channels), "adaptive threshold", stream, &s);
+  if (!rc) rc = check_adaptive_window(window_width, window_height);
+  if (rc) return rc;
+  if (window_width == 0 || window_height == 0) return clone_image(src, dst, width, height, channels, "adaptive threshold copy", s);
+  return launch_adaptive_threshold(src, dst, width, height, channels, window_width, window_height, bias,
+                                   update_bits(channels, update_mask), s);
+}
+
+int mb200_auto_threshold_image_dev(float *buf, size_t width, size_t height, int channels, int method,
+                                   double *threshold_percent, void *stream) {
+  cudaStream_t s;
+  int rc = prepare_dev(buf && valid_image(width, height, channels), "auto threshold", stream, &s);
+  if (!rc) rc = check_auto_threshold(width, height, method, threshold_percent);
+  if (rc) return rc;
+  unsigned counts[256];
+  rc = auto_threshold_histogram(buf, width * height, channels, counts, s);
+  if (rc) return rc;
+  const double threshold = auto_threshold_percent(counts, method);
+  const double t[4] = {65535.0 * threshold / 100.0, 0, 0, 0};         // BilevelImage(QuantumRange*threshold/100)
+  rc = launch_threshold(buf, width * height, channels, 0, t, s);
+  if (!rc) *threshold_percent = threshold;
+  return rc;
+}
+
+int mb200_range_threshold_image_dev(float *buf, size_t width, size_t height, int channels, double low_black,
+                                    double low_white, double high_white, double high_black, int per_channel,
+                                    unsigned update_mask, void *stream) {
+  cudaStream_t s;
+  int rc = prepare_dev(buf && valid_image(width, height, channels), "range threshold", stream, &s);
+  if (!rc) rc = check_range_threshold(channels);
+  if (rc) return rc;
+  const double t[6] = {low_black, low_white, high_white, high_black,
+                       65535.0 * perceptible_reciprocal(low_white - low_black),
+                       65535.0 * perceptible_reciprocal(high_black - high_white)};
+  return launch_threshold(buf, width * height, channels, 4, t, s, update_bits(channels, update_mask), per_channel != 0);
+}
+
+int mb200_perceptible_image_dev(float *buf, size_t width, size_t height, int channels, double epsilon,
+                                unsigned update_mask, void *stream) {
+  cudaStream_t s;
+  const int rc = prepare_dev(buf && valid_image(width, height, channels), "perceptible", stream, &s);
+  if (rc) return rc;
+  const double t[4] = {epsilon, 0, 0, 0};
+  return launch_threshold(buf, width * height, channels, 5, t, s, update_bits(channels, update_mask));
+}
+
+int mb200_adaptive_threshold_image(const float *src, float *dst, size_t w, size_t h, int ch, size_t window_width,
+                                   size_t window_height, double bias, unsigned update_mask) {
+  const int rc = check_adaptive_window(window_width, window_height);
+  if (rc) return rc;
+  return with_staging("adaptive threshold", src, w, h, ch, dst, w, h, [&](const float *s, float *d, cudaStream_t st) {
+    return mb200_adaptive_threshold_image_dev(s, d, w, h, ch, window_width, window_height, bias, update_mask, st);
+  });
+}
+
+int mb200_auto_threshold_image(float *buf, size_t w, size_t h, int ch, int method, double *threshold_percent) {
+  const int rc = check_auto_threshold(w, h, method, threshold_percent);
+  if (rc) return rc;
+  return in_place_host("auto threshold", buf, w, h, ch, [&](float *d, cudaStream_t st) {
+    return mb200_auto_threshold_image_dev(d, w, h, ch, method, threshold_percent, st);
+  });
+}
+
+int mb200_range_threshold_image(float *buf, size_t w, size_t h, int ch, double low_black, double low_white,
+                                double high_white, double high_black, int per_channel, unsigned update_mask) {
+  const int rc = check_range_threshold(ch);
+  if (rc) return rc;
+  return in_place_host("range threshold", buf, w, h, ch, [&](float *d, cudaStream_t st) {
+    return mb200_range_threshold_image_dev(d, w, h, ch, low_black, low_white, high_white, high_black, per_channel,
+                                           update_mask, st);
+  });
+}
+
+int mb200_perceptible_image(float *buf, size_t w, size_t h, int ch, double epsilon, unsigned update_mask) {
+  return in_place_host("perceptible", buf, w, h, ch, [&](float *d, cudaStream_t st) {
+    return mb200_perceptible_image_dev(d, w, h, ch, epsilon, update_mask, st);
+  });
+}
+
+}  // extern "C"
+
 // ---- SharpenImage / EdgeImage: effect.c builds a kernel inline and calls ConvolveImage ------------------------
 extern "C" {
 

@@ -17,9 +17,18 @@ __device__ __forceinline__ unsigned scale_quantum_to_map(float q) {
   return static_cast<unsigned>(q + 0.5f);
 }
 
+// quantum.h:113-124 ScaleQuantumToChar (Q16, HDRI): float division and addition, as the reference evaluates them
+__device__ __forceinline__ unsigned scale_quantum_to_char(float q) {
+  if (!(q > 0.0f)) return 0u;                       // NaN or <= 0
+  const float d = __fdiv_rn(q, 257.0f);
+  if (d >= 255.0f) return 255u;
+  return static_cast<unsigned>(__fadd_rn(d, 0.5f));
+}
+
 // One histogram per channel (sync == 0) or one shared, intensity-driven histogram (sync != 0): counts[c][bin].
+// CHAR_BINS: the intensity histogram of AutoThresholdImage (threshold.c:731), 256 bins of ScaleQuantumToChar.
 // Lanes of a warp that hit the same bin are merged before the atomic (images have long runs of equal values).
-template <int CH>
+template <int CH, bool CHAR_BINS = false>
 __global__ void __launch_bounds__(256) histogram_kernel(const float *__restrict__ buf, size_t npixels, int sync,
                                                         unsigned *__restrict__ counts) {
   const size_t i = static_cast<size_t>(blockIdx.x) * 256 + threadIdx.x;
@@ -39,7 +48,8 @@ __global__ void __launch_bounds__(256) histogram_kernel(const float *__restrict_
     if (CH > 1)          // Gray+Alpha: the green / blue accessors resolve to the gray sample (same expression on g,g,g)
       pixel = __dadd_rn(__dadd_rn(__dmul_rn(0.212656, red), __dmul_rn(0.715158, static_cast<double>(v[CH >= 3 ? 1 : 0]))),
                         __dmul_rn(0.072186, static_cast<double>(v[CH >= 3 ? 2 : 0])));
-    add(counts, scale_quantum_to_map(static_cast<float>(pixel)));        // ClampToQuantum (HDRI) == the float cast
+    const float quantum = static_cast<float>(pixel);                     // ClampToQuantum (HDRI) == the float cast
+    add(counts, CHAR_BINS ? scale_quantum_to_char(quantum) : scale_quantum_to_map(quantum));
   } else {
 #pragma unroll
     for (int c = 0; c < CH; ++c) add(counts + static_cast<size_t>(c) * kBins, scale_quantum_to_map(v[c]));

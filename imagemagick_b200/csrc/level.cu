@@ -238,24 +238,33 @@ int launch_range(const float *buf, size_t width, size_t height, int channels, un
   return e == cudaSuccess ? MB200_OK : cuda_fail(e, "range launch");
 }
 
-// The histogram pass of equalize.cuh into a fresh device buffer of nhist * kBins counts, read back into `counts`.
+template <bool CHAR_BINS>
+void launch_histogram(const float *buf, size_t npixels, int channels, int sync, unsigned *d_counts, unsigned grid,
+                      cudaStream_t s) {
+  switch (channels) {
+    case 1: histogram_kernel<1, CHAR_BINS><<<grid, 256, 0, s>>>(buf, npixels, sync, d_counts); break;
+    case 2: histogram_kernel<2, CHAR_BINS><<<grid, 256, 0, s>>>(buf, npixels, sync, d_counts); break;
+    case 3: histogram_kernel<3, CHAR_BINS><<<grid, 256, 0, s>>>(buf, npixels, sync, d_counts); break;
+    default: histogram_kernel<4, CHAR_BINS><<<grid, 256, 0, s>>>(buf, npixels, sync, d_counts); break;
+  }
+}
+
+// The histogram pass of equalize.cuh into a fresh device buffer of nhist * kBins counts, read back into `counts`;
+// char_bins: AutoThresholdImage's 256-bin intensity histogram (sync implied).
 int histogram_readback(const float *buf, size_t npixels, int channels, int sync, std::vector<unsigned> *counts,
-                       cudaStream_t s) {
+                       cudaStream_t s, bool char_bins = false) {
   unsigned grid;
   int rc = grid_of(npixels, 256, &grid, "histogram");
   if (rc) return rc;
+  if (char_bins) sync = 1;
   const int nhist = sync ? 1 : channels;
   unsigned *d_counts = nullptr;
   cudaError_t e = cudaMallocAsync(reinterpret_cast<void **>(&d_counts), sizeof(unsigned) * kBins * nhist, temp_pool(), s);
   if (e != cudaSuccess) return cuda_fail(e, "histogram: allocation");
   e = cudaMemsetAsync(d_counts, 0, sizeof(unsigned) * kBins * nhist, s);
   if (e == cudaSuccess) {
-    switch (channels) {
-      case 1: histogram_kernel<1><<<grid, 256, 0, s>>>(buf, npixels, sync, d_counts); break;
-      case 2: histogram_kernel<2><<<grid, 256, 0, s>>>(buf, npixels, sync, d_counts); break;
-      case 3: histogram_kernel<3><<<grid, 256, 0, s>>>(buf, npixels, sync, d_counts); break;
-      default: histogram_kernel<4><<<grid, 256, 0, s>>>(buf, npixels, sync, d_counts); break;
-    }
+    if (char_bins) launch_histogram<true>(buf, npixels, channels, sync, d_counts, grid, s);
+    else launch_histogram<false>(buf, npixels, channels, sync, d_counts, grid, s);
     count_launch();
     counts->assign(static_cast<size_t>(kBins) * nhist, 0u);
     e = cudaGetLastError();
@@ -451,6 +460,14 @@ int launch_identify_gray(const float *buf, size_t npixels, int channels, int *ty
   cudaFreeAsync(d_flags, s);
   if (e != cudaSuccess) return cuda_fail(e, "identify gray");
   *type = (flags & 1u) ? 0 : (flags & 2u) ? 1 : 2;
+  return MB200_OK;
+}
+
+int auto_threshold_histogram(const float *buf, size_t npixels, int channels, unsigned counts[256], void *stream) {
+  std::vector<unsigned> all;
+  const int rc = histogram_readback(buf, npixels, channels, 1, &all, static_cast<cudaStream_t>(stream), true);
+  if (rc) return rc;
+  std::copy(all.begin(), all.begin() + 256, counts);
   return MB200_OK;
 }
 

@@ -30,6 +30,7 @@ struct TuningKnobs {
   int no_rank1, no_morph_stream, no_resize_stream, resize_regular_h, no_fused_unsharp;
   int resize_fused, no_resize_fused;                                   // force the fused / the two-pass ResizeImage
   int conv2d_rows;                                                     // morph2d.cu: 0 automatic, else 8 / 4 / 2
+  int no_adaptive_tile;                                                // threshold.cu: force the direct family
 };
 TuningKnobs tuning_knobs();
 
@@ -44,6 +45,7 @@ enum LaunchFamily {
   kMorphDirect,                                                        // morph_direct.cu
   kDistort,                                                            // distort.cu
   kGeometry,                                                           // geometry.cu
+  kAdaptiveThresholdTile, kAdaptiveThresholdDirect,                    // threshold.cu
   kLaunchFamilies
 };
 void count_family(LaunchFamily family);
@@ -287,7 +289,19 @@ int launch_linear_stretch(float *buf, size_t width, size_t height, int channels,
 int launch_gamma(float *buf, size_t npixels, int channels, double gamma, unsigned update_mask, void *stream);
 int launch_identify_gray(const float *buf, size_t npixels, int channels, int *type, void *stream);
 
-// threshold.c point operators in place; op: 0 bilevel (t[0]), 1 black, 2 white (t = r,g,b,a), 3 clamp
-int launch_threshold(float *buf, size_t npixels, int channels, int op, const double *thresholds, void *stream);
+// threshold.c point operators in place; op: 0 bilevel (t[0]), 1 black, 2 white (t = r,g,b,a), 3 clamp (every channel);
+// 4 range (t = low black, low white, high white, high black, QuantumRange*PerceptibleReciprocal(lw-lb),
+// QuantumRange*PerceptibleReciprocal(hb-hw); per_channel: the sample instead of the intensity), 5 perceptible (t[0] =
+// epsilon) on the channels of update_mask
+int launch_threshold(float *buf, size_t npixels, int channels, int op, const double *thresholds, void *stream,
+                     unsigned update_mask = 0xfu, bool per_channel = false);
+// AutoThresholdImage's histogram (threshold.c:717-735): 256 bins of ScaleQuantumToChar(ClampToQuantum(intensity)), read
+// back (synchronises the stream)
+int auto_threshold_histogram(const float *buf, size_t npixels, int channels, unsigned counts[256], void *stream);
+// threshold.cu: AutoThresholdImage's threshold (percent) of `method` from that histogram, in the reference's arithmetic
+double auto_threshold_percent(const unsigned counts[256], int method);
+// threshold.cu: AdaptiveThresholdImage (threshold.c:182) out of place on the channels of update_mask (the others copy)
+int launch_adaptive_threshold(const float *src, float *dst, size_t width, size_t height, int channels, size_t w, size_t h,
+                              double bias, unsigned update_mask, void *stream);
 
 }  // namespace mb200

@@ -37,10 +37,13 @@ __global__ void __launch_bounds__(256) unsharp_tail_kernel(const float *__restri
 // :2518, ClampImage :1087).  Every channel (alpha included) is compared through the pixel's intensity
 // (pixel.c:2356, Rec709Luma on an sRGB / gray image), evaluated exactly as the reference does: three
 // products summed left to right in double with no contraction, so the comparison -- and therefore the
-// result -- is bit-identical.  op: 0 bilevel, 1 black, 2 white, 3 clamp.
+// result -- is bit-identical.  op: 0 bilevel, 1 black, 2 white, 3 clamp, on every channel; 4 RangeThresholdImage
+// (:2377) and 5 PerceptibleImage (:2092) on the channels of `update`.
 struct ThresholdArgs {
-  double t[4];     // bilevel: t[0]; black / white: red, green, blue, alpha
+  double t[6];     // bilevel, perceptible: t[0]; black / white: red, green, blue, alpha; range: see launch_threshold
   int op;
+  unsigned update;
+  bool per_channel;
 };
 
 template <int CH>
@@ -63,6 +66,13 @@ __global__ void __launch_bounds__(256) threshold_kernel(float *__restrict__ buf,
       if (p < 0.0) v[c] = 0.0f;
       else if (p >= kQR) v[c] = 65535.0f;
     }
+  } else if (a.op == 5) {                              // PerceptibleThreshold (:2080)
+#pragma unroll
+    for (int c = 0; c < CH; ++c) {
+      if (!((a.update >> c) & 1u)) continue;
+      const double q = static_cast<double>(v[c]), sign = q < 0.0 ? -1.0 : 1.0;
+      if (!(__dmul_rn(sign, q) >= a.t[0])) v[c] = static_cast<float>(__dmul_rn(sign, a.t[0]));
+    }
   } else {
     const double red = static_cast<double>(v[0]);
     double pixel = red;
@@ -71,6 +81,18 @@ __global__ void __launch_bounds__(256) threshold_kernel(float *__restrict__ buf,
       const double blue = CH >= 3 ? static_cast<double>(v[CH >= 3 ? 2 : 0]) : red;
       pixel = __dadd_rn(__dadd_rn(__dmul_rn(0.212656, red), __dmul_rn(0.715158, green)), __dmul_rn(0.072186, blue));
     }
+    if (a.op == 4) {                                   // :2446-2464, ClampToQuantum = the float cast (HDRI)
+#pragma unroll
+      for (int c = 0; c < CH; ++c) {
+        if (!((a.update >> c) & 1u)) continue;
+        if (a.per_channel) pixel = static_cast<double>(v[c]);
+        if (pixel < a.t[0]) v[c] = 0.0f;
+        else if (pixel >= a.t[0] && pixel < a.t[1]) v[c] = static_cast<float>(__dmul_rn(a.t[4], __dsub_rn(pixel, a.t[0])));
+        else if (pixel >= a.t[1] && pixel <= a.t[2]) v[c] = 65535.0f;
+        else if (pixel > a.t[2] && pixel <= a.t[3]) v[c] = static_cast<float>(__dmul_rn(a.t[5], __dsub_rn(a.t[3], pixel)));
+        else v[c] = 0.0f;
+      }
+    } else {
 #pragma unroll
     for (int c = 0; c < CH; ++c) {
       const bool is_alpha = (CH == 2 || CH == 4) && c == CH - 1;
@@ -78,6 +100,7 @@ __global__ void __launch_bounds__(256) threshold_kernel(float *__restrict__ buf,
       if (a.op == 0) v[c] = pixel <= t ? 0.0f : 65535.0f;
       else if (a.op == 1) { if (pixel < t) v[c] = 0.0f; }
       else { if (pixel > t) v[c] = 65535.0f; }
+    }
     }
   }
   if (CH == 4) reinterpret_cast<float4 *>(buf)[i] = make_float4(v[0], v[1], v[2], v[CH - 1]);
@@ -314,11 +337,14 @@ int launch_composite_lighten(float *canvas, const float *source, size_t npixels,
   return launch_composite<1>(canvas, source, npixels, channels, stream);
 }
 
-int launch_threshold(float *buf, size_t npixels, int channels, int op, const double *thresholds, void *stream) {
+int launch_threshold(float *buf, size_t npixels, int channels, int op, const double *thresholds, void *stream,
+                     unsigned update_mask, bool per_channel) {
   if (npixels == 0) return MB200_OK;
   ThresholdArgs a{};
-  for (int k = 0; k < 4; ++k) a.t[k] = thresholds ? thresholds[k] : 0.0;
+  for (int k = 0; k < (op == 4 ? 6 : 4); ++k) a.t[k] = thresholds ? thresholds[k] : 0.0;
   a.op = op;
+  a.update = update_mask;
+  a.per_channel = per_channel;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const size_t blocks = (npixels + 255) / 256;
   if (blocks > 0x7fffffffull) return fail(MB200_EINVAL, "threshold: image too large");

@@ -101,6 +101,7 @@ const KnobSpec kKnobs[] = {
     {"no_resize_stream", &TuningKnobs::no_resize_stream, 0, any_value, kSwitch},
     {"no_fused_unsharp", &TuningKnobs::no_fused_unsharp, 0, any_value, kSwitch},
     {"no_resize_fused", &TuningKnobs::no_resize_fused, 0, any_value, kSwitch},
+    {"no_adaptive_tile", &TuningKnobs::no_adaptive_tile, 0, any_value, kSwitch},
     // opt-in path that measured slower than the default
     {"resize_regular_h", &TuningKnobs::resize_regular_h, 0, any_value, kSwitch},
     // the fused ResizeImage wherever it applies, also below the automatic size threshold
@@ -144,7 +145,7 @@ const char *const kFamilyNames[kLaunchFamilies] = {
     "resize_v_stream_launches", "resize_h_tma_launches", "resize_h_stream_launches", "resize_fused_launches",
     "resize_regular_launches", "resize_gather_launches", "conv2d_dense_r8_launches", "conv2d_dense_r4_launches",
     "conv2d_dense_r2_launches", "morph2d_launches", "minmax2d_launches", "morph_stream_launches", "morph_direct_launches",
-    "distort_launches", "geometry_launches"};
+    "distort_launches", "geometry_launches", "adaptive_threshold_tile_launches", "adaptive_threshold_direct_launches"};
 std::atomic<unsigned long long> g_family_launches[kLaunchFamilies];
 int family_index(const char *name) {
   for (int f = 0; f < kLaunchFamilies; ++f)

@@ -13,9 +13,10 @@
           --wrap=ContrastStretchImage,--wrap=NormalizeImage,--wrap=LinearStretchImage,--wrap=LevelImage,\
           --wrap=LevelizeImage,--wrap=MinMaxStretchImage,--wrap=GammaImage,--wrap=DistortImage,--wrap=RotateImage,\
           --wrap=FlipImage,--wrap=FlopImage,--wrap=TransposeImage,--wrap=TransverseImage,--wrap=IntegralRotateImage,\
-          --wrap=CropImage,--wrap=CropImageToTiles,--wrap=ShaveImage,--wrap=RollImage,--wrap=AutoOrientImage
+          --wrap=CropImage,--wrap=CropImageToTiles,--wrap=ShaveImage,--wrap=RollImage,--wrap=AutoOrientImage,\
+          --wrap=AdaptiveThresholdImage,--wrap=AutoThresholdImage,--wrap=RangeThresholdImage,--wrap=PerceptibleImage
   and every caller of those exported functions (effect.c:765/1709/1170/4256, morphology.c:4129,
-  resize.c:3761, colorspace.c:1751, threshold.c:805/927/2518/1087, effect.c:1308/2013, visual-effects.c:3515,
+  resize.c:3761, colorspace.c:1751, threshold.c:805/927/2518/1087/182/660/2377/2092, effect.c:1308/2013, visual-effects.c:3515,
   enhance.c:1370/3461/2474/1544/4130/3347/2913/3062/2322, histogram.c:927, statistic.c:1064) reaches __wrap_X below.  Each wrapper follows the accelerate
   hook contract of effect.c:783-787 / resize.c:3818-3826: try the GPU; if the image is not
   eligible or the GPU path declines (returns NULL / MagickFalse without raising), run the stock
@@ -42,7 +43,9 @@
 /* update_mask == NULL: every channel must carry its default traits (no `-channel` selection).  Otherwise unselected
    channels (Copy trait, pixel.c:6338-6393 SetPixelChannelMask) are accepted and reported: bit c set = channel c is updated. */
 /* The channel layout test alone, whatever the virtual-pixel method (DistortImage serves several). */
-static int b200_layout_masked(const Image *image, unsigned *update_mask)
+/* single_stage: the operator reads each source sample of a channel only for that channel's result, so an unselected
+   alpha channel feeds nothing and is simply copied (the multi-stage rule below does not apply). */
+static int b200_layout_traits(const Image *image, unsigned *update_mask, int single_stage)
 {
   const size_t n = GetPixelChannels(image);
   const MagickBooleanType gray = (image->colorspace == GRAYColorspace) ||
@@ -71,7 +74,8 @@ static int b200_layout_masked(const Image *image, unsigned *update_mask)
        resize passes), so the later stages weight the colour channels with the ORIGINAL alpha instead of the filtered
        one: the selected channels then depend on the selection and a final restore pass cannot reproduce them.  Such
        selections stay on the CPU path; with alpha selected (or no alpha) the unselected channels feed nothing. */
-    if (image->alpha_trait != UndefinedPixelTrait && mask != ((1u << n) - 1u) && (mask >> (n - 1) & 1u) == 0) return 0;
+    if (!single_stage && image->alpha_trait != UndefinedPixelTrait && mask != ((1u << n) - 1u) &&
+        (mask >> (n - 1) & 1u) == 0) return 0;
   }
   if (gray != MagickFalse) {
     if (n == 1 && image->alpha_trait == UndefinedPixelTrait) return 1;
@@ -88,12 +92,18 @@ static int b200_layout_masked(const Image *image, unsigned *update_mask)
   return 0;
 }
 
-static int b200_channels_masked(const Image *image, unsigned *update_mask)
+static int b200_layout_masked(const Image *image, unsigned *update_mask)
+{ return b200_layout_traits(image, update_mask, 0); }
+
+static int b200_channels_stage(const Image *image, unsigned *update_mask, int single_stage)
 {
   if ((GetImageVirtualPixelMethod(image) != UndefinedVirtualPixelMethod) &&
       (GetImageVirtualPixelMethod(image) != EdgeVirtualPixelMethod)) return 0;
-  return b200_layout_masked(image, update_mask);
+  return b200_layout_traits(image, update_mask, single_stage);
 }
+
+static int b200_channels_masked(const Image *image, unsigned *update_mask)
+{ return b200_channels_stage(image, update_mask, 0); }
 
 static int b200_channels(const Image *image) { return b200_channels_masked(image, (unsigned *) NULL); }
 
@@ -180,12 +190,13 @@ typedef int (*same_size_op)(const float *, float *, size_t, size_t, int, const v
 
 /* src pixels -> new image through `op`; NULL == declined (caller falls back to the CPU).  allow_mask 1: the operator hands
    Copy-trait channels through from its source, so a -channel selection is served by one extra point pass; 2: the
-   operator ignores the selection (it computes the same channels whatever their traits), so it is served as is. */
+   operator ignores the selection (it computes the same channels whatever their traits), so it is served as is; 3: as 1
+   for a single-stage operator, whose unselected alpha channel feeds nothing (b200_layout_traits). */
 static Image *run_same_size_masked(const Image *image, same_size_op op, const void *args, int allow_mask,
                                    ExceptionInfo *exception)
 {
   unsigned update_mask = 0xfu;
-  const int ch = allow_mask ? b200_channels_masked(image, &update_mask) : b200_channels(image);
+  const int ch = allow_mask ? b200_channels_stage(image, &update_mask, allow_mask == 3) : b200_channels(image);
   const float *p;
   Quantum *q;
   Image *out;
@@ -200,7 +211,7 @@ static Image *run_same_size_masked(const Image *image, same_size_op op, const vo
       q = GetAuthenticPixels(out, 0, 0, out->columns, out->rows, attempt);
       if (q == (Quantum *) NULL || b200_cache_pixels(out, ch, attempt) != (float *) q ||
           op(p, (float *) q, image->columns, image->rows, ch, args) != MB200_OK ||
-          (allow_mask == 1 && (update_mask & ((1u << ch) - 1u)) != ((1u << ch) - 1u) &&
+          ((allow_mask == 1 || allow_mask == 3) && (update_mask & ((1u << ch) - 1u)) != ((1u << ch) - 1u) &&
            mb200_restore_channels((float *) q, p, image->columns, image->rows, ch, update_mask) != MB200_OK) ||
           SyncAuthenticPixels(out, attempt) == MagickFalse)
         out = DestroyImage(out);
@@ -857,6 +868,113 @@ MagickBooleanType B200AccelerateWhiteThresholdImage(Image *image, const char *th
 MagickBooleanType B200AccelerateClampImage(Image *image, ExceptionInfo *exception)
 { return run_threshold(image, 3, 0.0, (const char *) NULL, exception); }
 
+/* AdaptiveThresholdImage (threshold.c:182): edge / undefined virtual pixels; Copy-trait channels take the source sample,
+   which the restore pass of run_same_size_masked puts back.  width or height 0 (a plain clone) and windows beyond the
+   library's limit decline. */
+typedef struct { size_t width, height; double bias; } adaptive_threshold_args;
+static int op_adaptive_threshold(const float *s, float *d, size_t w, size_t h, int ch, const void *a)
+{
+  const adaptive_threshold_args *t = (const adaptive_threshold_args *) a;
+  return mb200_adaptive_threshold_image(s, d, w, h, ch, t->width, t->height, t->bias, 0xfu);
+}
+
+Image *B200AccelerateAdaptiveThresholdImage(const Image *image, const size_t width, const size_t height, const double bias,
+                                            ExceptionInfo *exception)
+{
+  adaptive_threshold_args a;
+  if (width == 0 || height == 0) return (Image *) NULL;
+  a.width = width; a.height = height; a.bias = bias;
+  return run_same_size_masked(image, op_adaptive_threshold, &a, 3, exception);
+}
+
+/* In place on the Update channels of a single-stage operator (op 0 AutoThreshold, 1 RangeThreshold, 2 Perceptible). */
+typedef struct { int op, method, per_channel; double x[4]; double threshold; } threshold_args;
+static MagickBooleanType run_threshold_masked(Image *image, threshold_args *a)
+{
+  MagickBooleanType ok = MagickFalse;
+  unsigned update_mask = 0;
+  const int ch = b200_layout_traits(image, &update_mask, 1);     /* point operators: no virtual pixels */
+  Quantum *q;
+  int rc = MB200_EINVAL;
+  if (ch == 0 || mb200_device_count() <= 0) return MagickFalse;
+  {
+    B200_ATTEMPT_BEGIN;
+    q = GetAuthenticPixels(image, 0, 0, image->columns, image->rows, attempt);
+    if (q != (Quantum *) NULL && b200_cache_pixels(image, ch, attempt) == (float *) q) {
+      float *buf = (float *) q;
+      const size_t w = image->columns, h = image->rows;
+      switch (a->op) {
+        case 0: rc = mb200_auto_threshold_image(buf, w, h, ch, a->method, &a->threshold); break;
+        case 1:
+          rc = mb200_range_threshold_image(buf, w, h, ch, a->x[0], a->x[1], a->x[2], a->x[3], a->per_channel, update_mask);
+          break;
+        default: rc = mb200_perceptible_image(buf, w, h, ch, a->x[0], update_mask); break;
+      }
+    }
+    /* on failure nothing was written back: the CPU path starts from the same pixels */
+    if (rc == MB200_OK && SyncAuthenticPixels(image, attempt) != MagickFalse) ok = MagickTrue;
+    B200_ATTEMPT_END;
+  }
+  return ok;
+}
+
+/* AutoThresholdImage (threshold.c:660): the Rec709Luma intensity histogram of an sRGB-compatible or gray image, then
+   BilevelImage under the default channel mask (its call stays inside threshold.o), the "auto-threshold:threshold"
+   property and BilevelImage's sRGB tag.  The auto-threshold:verbose report, a channel mask (BilevelImage would then
+   threshold each channel on its own value), other intensity methods and linear RGB / LinearGRAY images decline. */
+MagickBooleanType B200AccelerateAutoThresholdImage(Image *image, const AutoThresholdMethod method, ExceptionInfo *exception)
+{
+  threshold_args a;
+  char property[MagickPathExtent];
+  if (GetImageArtifact(image, "auto-threshold:verbose") != (const char *) NULL) return MagickFalse;
+  if (image->channel_mask != AllChannels || default_intensity(image) == MagickFalse) return MagickFalse;
+  if (image->colorspace == RGBColorspace || image->colorspace == LinearGRAYColorspace) return MagickFalse;
+  if (b200_layout_masked(image, (unsigned *) NULL) == 0) return MagickFalse;     /* every channel with its default traits */
+  (void) memset(&a, 0, sizeof(a));
+  a.op = 0;
+  a.method = (method == KapurThresholdMethod) ? MB200_KapurThresholdMethod :
+             (method == TriangleThresholdMethod) ? MB200_TriangleThresholdMethod : MB200_OTSUThresholdMethod;
+  if (run_threshold_masked(image, &a) == MagickFalse) return MagickFalse;
+  (void) FormatLocaleString(property, MagickPathExtent, "%g%%", a.threshold);
+  (void) SetImageProperty(image, "auto-threshold:threshold", property, exception);
+  if (IsGrayColorspace(image->colorspace) == MagickFalse)
+    (void) SetImageColorspace(image, sRGBColorspace, exception);              /* threshold.c:827 */
+  return MagickTrue;
+}
+
+/* RangeThresholdImage (threshold.c:2377): a gray image is first transformed to sRGB (:2407) through the wrapped
+   TransformImageColorspace; the default channel mask thresholds on the intensity (Rec709Luma, not on a linear RGB
+   image), a selection on each channel's own sample. */
+MagickBooleanType B200AccelerateRangeThresholdImage(Image *image, const double low_black, const double low_white,
+                                                    const double high_white, const double high_black,
+                                                    ExceptionInfo *exception)
+{
+  threshold_args a;
+  const int per_channel = image->channel_mask != AllChannels ? 1 : 0;
+  if (mb200_device_count() <= 0) return MagickFalse;
+  if (!per_channel && (default_intensity(image) == MagickFalse || image->colorspace == RGBColorspace)) return MagickFalse;
+  {
+    unsigned mask = 0;
+    if (b200_layout_traits(image, &mask, 1) == 0) return MagickFalse;      /* before the transform */
+  }
+  if (IsGrayColorspace(image->colorspace) != MagickFalse &&
+      TransformImageColorspace(image, sRGBColorspace, exception) == MagickFalse) return MagickFalse;
+  (void) memset(&a, 0, sizeof(a));
+  a.op = 1; a.per_channel = per_channel;
+  a.x[0] = low_black; a.x[1] = low_white; a.x[2] = high_white; a.x[3] = high_black;
+  return run_threshold_masked(image, &a);
+}
+
+/* PerceptibleImage (threshold.c:2092) on the Update channels; the PseudoClass colormap branch declines. */
+MagickBooleanType B200AcceleratePerceptibleImage(Image *image, const double epsilon, ExceptionInfo *exception)
+{
+  threshold_args a;
+  (void) exception;
+  (void) memset(&a, 0, sizeof(a));
+  a.op = 2; a.x[0] = epsilon;
+  return run_threshold_masked(image, &a);
+}
+
 /* ---- SharpenImage / EdgeImage (effect.c:3991, :1520): inline kernel + ConvolveImage -------------------------- */
 static int op_sharpen(const float *s, float *d, size_t w, size_t h, int ch, const void *a)
 { const blur_args *b = (const blur_args *) a; return mb200_sharpen_image(s, d, w, h, ch, b->radius, b->sigma); }
@@ -1292,6 +1410,11 @@ extern MagickBooleanType __real_BilevelImage(Image *, const double, ExceptionInf
 extern MagickBooleanType __real_BlackThresholdImage(Image *, const char *, ExceptionInfo *);
 extern MagickBooleanType __real_WhiteThresholdImage(Image *, const char *, ExceptionInfo *);
 extern MagickBooleanType __real_ClampImage(Image *, ExceptionInfo *);
+extern Image *__real_AdaptiveThresholdImage(const Image *, const size_t, const size_t, const double, ExceptionInfo *);
+extern MagickBooleanType __real_AutoThresholdImage(Image *, const AutoThresholdMethod, ExceptionInfo *);
+extern MagickBooleanType __real_RangeThresholdImage(Image *, const double, const double, const double, const double,
+                                                    ExceptionInfo *);
+extern MagickBooleanType __real_PerceptibleImage(Image *, const double, ExceptionInfo *);
 
 static long b200_hits = 0, b200_fallbacks = 0;          /* updated with atomic adds: the entry points are re-entrant */
 static int b200_enabled = -1;       /* -1: not yet read from the environment */
@@ -1387,6 +1510,32 @@ MagickBooleanType __wrap_ClampImage(Image *image, ExceptionInfo *exception)
 {
   TRY_BOOL(B200AccelerateClampImage(image, exception));
   return __real_ClampImage(image, exception);
+}
+
+Image *__wrap_AdaptiveThresholdImage(const Image *image, const size_t width, const size_t height, const double bias,
+                                     ExceptionInfo *exception)
+{
+  TRY(B200AccelerateAdaptiveThresholdImage(image, width, height, bias, exception));
+  return __real_AdaptiveThresholdImage(image, width, height, bias, exception);
+}
+
+MagickBooleanType __wrap_AutoThresholdImage(Image *image, const AutoThresholdMethod method, ExceptionInfo *exception)
+{
+  TRY_BOOL(B200AccelerateAutoThresholdImage(image, method, exception));
+  return __real_AutoThresholdImage(image, method, exception);
+}
+
+MagickBooleanType __wrap_RangeThresholdImage(Image *image, const double low_black, const double low_white,
+                                             const double high_white, const double high_black, ExceptionInfo *exception)
+{
+  TRY_BOOL(B200AccelerateRangeThresholdImage(image, low_black, low_white, high_white, high_black, exception));
+  return __real_RangeThresholdImage(image, low_black, low_white, high_white, high_black, exception);
+}
+
+MagickBooleanType __wrap_PerceptibleImage(Image *image, const double epsilon, ExceptionInfo *exception)
+{
+  TRY_BOOL(B200AcceleratePerceptibleImage(image, epsilon, exception));
+  return __real_PerceptibleImage(image, epsilon, exception);
 }
 
 Image *__wrap_SharpenImage(const Image *image, const double radius, const double sigma, ExceptionInfo *exception)

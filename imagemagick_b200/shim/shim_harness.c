@@ -54,6 +54,11 @@ extern MagickBooleanType __real_LinearStretchImage(Image *, const double, const 
 extern MagickBooleanType __real_LevelImage(Image *, const double, const double, const double, ExceptionInfo *);
 extern MagickBooleanType __real_LevelizeImage(Image *, const double, const double, const double, ExceptionInfo *);
 extern MagickBooleanType __real_GammaImage(Image *, const double, ExceptionInfo *);
+extern Image *__real_AdaptiveThresholdImage(const Image *, const size_t, const size_t, const double, ExceptionInfo *);
+extern MagickBooleanType __real_AutoThresholdImage(Image *, const AutoThresholdMethod, ExceptionInfo *);
+extern MagickBooleanType __real_RangeThresholdImage(Image *, const double, const double, const double, const double,
+                                                    ExceptionInfo *);
+extern MagickBooleanType __real_PerceptibleImage(Image *, const double, ExceptionInfo *);
 extern long B200ShimHits(void), B200ShimFallbacks(void);
 extern void B200ShimEnable(int);
 
@@ -176,6 +181,56 @@ static int level_case(const char *name, int bar, const Image *src, int op, doubl
          (int) GetPixelChannels(b), bad || d > bar ? "  FAIL" : "");
   a = DestroyImage(a); b = DestroyImage(b);
   return bad || d > bar;
+}
+
+/* op: 0 AdaptiveThreshold (x = width, y = height, z = bias), 1 AutoThreshold (x = method), 2 RangeThreshold (x, y, z, t),
+   3 Perceptible (x = epsilon) on a clone of `src` (channel mask `mask` unless negative), through the shim and through
+   __real_: the pixels bit for bit, the channel count, the colourspace, the type and the "auto-threshold:threshold"
+   property must agree; with `expect_fallback` the shim must have declined, otherwise it must have served the call.
+   1 on failure. */
+static int threshold_case(const char *name, const Image *src, int op, double x, double y, double z, double t, long mask,
+                          int expect_fallback, ExceptionInfo *ex)
+{
+  Image *a = CloneImage(src, 0, 0, MagickTrue, ex), *b = CloneImage(src, 0, 0, MagickTrue, ex), *ra = a, *rb = b;
+  const long fb = B200ShimFallbacks(), hits = B200ShimHits();
+  MagickBooleanType oka = MagickFalse, okb = MagickFalse;
+  const char *pa, *pb;
+  long d = 0;
+  int bad = 0;
+  if (mask >= 0) { (void) SetPixelChannelMask(a, (ChannelType) mask); (void) SetPixelChannelMask(b, (ChannelType) mask); }
+  switch (op) {
+    case 0:
+      ra = AdaptiveThresholdImage(a, (size_t) x, (size_t) y, z, ex);
+      B200ShimEnable(0); rb = __real_AdaptiveThresholdImage(b, (size_t) x, (size_t) y, z, ex); B200ShimEnable(1);
+      oka = ra != NULL ? MagickTrue : MagickFalse; okb = rb != NULL ? MagickTrue : MagickFalse;
+      break;
+    case 1:
+      oka = AutoThresholdImage(a, (AutoThresholdMethod) (int) x, ex);
+      B200ShimEnable(0); okb = __real_AutoThresholdImage(b, (AutoThresholdMethod) (int) x, ex); B200ShimEnable(1);
+      break;
+    case 2:
+      oka = RangeThresholdImage(a, x, y, z, t, ex);
+      B200ShimEnable(0); okb = __real_RangeThresholdImage(b, x, y, z, t, ex); B200ShimEnable(1);
+      break;
+    default:
+      oka = PerceptibleImage(a, x, ex);
+      B200ShimEnable(0); okb = __real_PerceptibleImage(b, x, ex); B200ShimEnable(1);
+      break;
+  }
+  if (oka == MagickFalse || okb == MagickFalse || GetPixelChannels(ra) != GetPixelChannels(rb) ||
+      ra->colorspace != rb->colorspace || ra->type != rb->type) bad = 1;
+  else {
+    pa = GetImageProperty(ra, "auto-threshold:threshold", ex); pb = GetImageProperty(rb, "auto-threshold:threshold", ex);
+    if ((pa == NULL) != (pb == NULL) || (pa != NULL && strcmp(pa, pb) != 0)) bad = 1;
+    d = compare(ra, rb, ex);
+  }
+  if (mb200_device_count() > 0 && (expect_fallback ? B200ShimFallbacks() <= fb : B200ShimHits() <= hits)) bad = 1;
+  printf("%-34s max ULP %ld (bar 0) channels %d/%d%s\n", name, d, oka ? (int) GetPixelChannels(ra) : 0,
+         okb ? (int) GetPixelChannels(rb) : 0, bad || d > 0 ? "  FAIL" : "");
+  if (ra != NULL && ra != a) ra = DestroyImage(ra);
+  if (rb != NULL && rb != b) rb = DestroyImage(rb);
+  a = DestroyImage(a); b = DestroyImage(b);
+  return bad || d > 0;
 }
 
 /* DistortImage (method >= 0) / RotateImage (method < 0) on `src` through the shim and through __real_: pixels (bit
@@ -578,6 +633,36 @@ int main(void)
     CHECK("BilevelImage -channel RGB (declines)", 0, a, b);
     if (mb200_device_count() > 0 && B200ShimFallbacks() <= fb) { printf("FAIL: per-channel threshold was not declined\n"); failures++; }
     (void) SetPixelChannelMask(rgb, DefaultChannels);
+  }
+  {
+    /* threshold.c: AdaptiveThreshold (-lat), AutoThreshold, RangeThreshold, Perceptible; bit exact */
+    const long hits0 = B200ShimHits();
+    const long rgb_mask = RedChannel | GreenChannel | BlueChannel;
+    Image *gray = CloneImage(rgb, 0, 0, MagickTrue, ex), *t;
+    (void) __real_TransformImageColorspace(gray, GRAYColorspace, ex);
+    failures += threshold_case("AdaptiveThreshold 15x15+5% RGBA", rgba, 0, 15, 15, 0.05 * QuantumRange, 0, -1, 0, ex);
+    failures += threshold_case("AdaptiveThreshold 4x6-500 RGB", rgb, 0, 4, 6, -500.0, 0, -1, 0, ex);
+    failures += threshold_case("AdaptiveThreshold 7x5 -channel RGB", rgba, 0, 7, 5, 300.0, 0, rgb_mask, 0, ex);
+    failures += threshold_case("AdaptiveThreshold 51x51 gray", gray, 0, 51, 51, 0.0, 0, -1, 0, ex);
+    failures += threshold_case("AutoThreshold OTSU RGBA", rgba, 1, OTSUThresholdMethod, 0, 0, 0, -1, 0, ex);
+    failures += threshold_case("AutoThreshold Kapur RGB", rgb, 1, KapurThresholdMethod, 0, 0, 0, -1, 0, ex);
+    failures += threshold_case("AutoThreshold Triangle gray", gray, 1, TriangleThresholdMethod, 0, 0, 0, -1, 0, ex);
+    failures += threshold_case("RangeThreshold RGBA", rgba, 2, 10000, 20000, 40000, 50000, -1, 0, ex);
+    failures += threshold_case("RangeThreshold -channel RGB RGBA", rgba, 2, 10000, 20000, 40000, 50000, rgb_mask, 0, ex);
+    failures += threshold_case("RangeThreshold gray -> sRGB", gray, 2, 10000, 10000, 40000, 50000, -1, 0, ex);
+    failures += threshold_case("Perceptible 30000 RGBA", rgba, 3, 30000.0, 0, 0, 0, -1, 0, ex);
+    failures += threshold_case("Perceptible -channel RGB RGBA", rgba, 3, 30000.0, 0, 0, 0, rgb_mask, 0, ex);
+    if (mb200_device_count() > 0 && B200ShimHits() - hits0 < 12) { printf("FAIL: threshold operators did not reach the GPU path\n"); failures++; }
+    failures += threshold_case("fallback: AdaptiveThreshold 0x5", rgba, 0, 0, 5, 0.0, 0, -1, 1, ex);
+    t = CloneImage(rgb, 0, 0, MagickTrue, ex);
+    t->colorspace = RGBColorspace;
+    failures += threshold_case("fallback: AutoThreshold linear RGB", t, 1, OTSUThresholdMethod, 0, 0, 0, -1, 1, ex);
+    t = DestroyImage(t);
+    t = CloneImage(rgb, 0, 0, MagickTrue, ex);
+    (void) SetImageType(t, PaletteType, ex);
+    failures += threshold_case("fallback: Perceptible PseudoClass", t, 3, 1000.0, 0, 0, 0, -1, 1, ex);
+    t = DestroyImage(t);
+    gray = DestroyImage(gray);
   }
   {
     /* a declined case must silently take the CPU path: tiled virtual pixels are not eligible */

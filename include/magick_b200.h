@@ -204,7 +204,8 @@ MB200_API int mb200_probe_fp64_fma_rate(double *fma_per_second);
    ignored: the default applies).  Launch counters per kernel family, readable like "conv_mma_launches":
    "conv_pair_launches", "conv_pair_async_launches", "conv_generic_launches", "resize_v_stream_launches",
    "resize_h_tma_launches", "resize_h_stream_launches", "resize_fused_launches", "resize_regular_launches",
-   "resize_gather_launches". */
+   "resize_gather_launches", "adaptive_threshold_tile_launches", "adaptive_threshold_direct_launches" (with the switch
+   "no_adaptive_tile", which sends AdaptiveThresholdImage to its direct family). */
 MB200_API int mb200_set_option(const char *name, int value);
 MB200_API int mb200_get_option(const char *name, int *value);
 
@@ -579,6 +580,37 @@ MB200_API int mb200_white_threshold_image_dev(float *buf, size_t width, size_t h
     int colorspace, const char *thresholds, void *stream);
 /* ClampImage (:1087): ClampPixel on every channel (HDRI: below 0 -> 0, >= QuantumRange -> QuantumRange). */
 MB200_API int mb200_clamp_image_dev(float *buf, size_t width, size_t height, int channels, void *stream);
+/* AdaptiveThresholdImage (:182), out of place `src` -> `dst` (no overlap), bit exact: every channel of `update_mask`
+   := (double) centre <= mean ? 0 : QuantumRange, mean = S / (double) (width*height) + bias, where S is the reference's
+   running double sum of the width x height window (origin -(width/2), -(height/2); edge virtual pixels), updated in the
+   reference's order along each row (a NaN or +-inf that enters it stays for the rest of the row).  The other channels
+   (the Copy trait) copy the source.  `bias` is in quantum units (the CLI's `-lat WxH+b%` passes QuantumRange*b/100).
+   width == 0 or height == 0 copies `src`.  Windows wider or taller than MB200_ADAPTIVE_THRESHOLD_MAX_WINDOW give
+   MB200_EUNSUPPORTED with `dst` untouched. */
+#define MB200_ADAPTIVE_THRESHOLD_MAX_WINDOW 4096
+MB200_API int mb200_adaptive_threshold_image_dev(const float *src, float *dst, size_t width, size_t height, int channels,
+    size_t window_width, size_t window_height, double bias, unsigned update_mask, void *stream);
+/* MagickCore/threshold.h AutoThresholdMethod -- same numeric values (Undefined means OTSU) */
+typedef enum {
+  MB200_UndefinedThresholdMethod = 0, MB200_KapurThresholdMethod, MB200_OTSUThresholdMethod,
+  MB200_TriangleThresholdMethod
+} mb200_auto_threshold_method;
+/* AutoThresholdImage (:660), in place, default channel mask: the 256-bin histogram of
+   ScaleQuantumToChar(ClampToQuantum(intensity)), the threshold of `method` computed on the host in the reference's order
+   with the same libm calls, then BilevelImage at QuantumRange*threshold/100.  `threshold_percent` receives the threshold
+   (the "auto-threshold:threshold" property is its "%g%%").  Bit exact.  Images of 2^32 pixels or more give
+   MB200_EUNSUPPORTED. */
+MB200_API int mb200_auto_threshold_image_dev(float *buf, size_t width, size_t height, int channels, int method,
+    double *threshold_percent, void *stream);
+/* RangeThresholdImage (:2377), in place on the channels of `update_mask`: the five-way branch of :2446-2464 on the
+   pixel's intensity (per_channel == 0: the default channel mask) or on the channel's own sample (per_channel != 0: a
+   `-channel` selection).  Bit exact.  Gray images (1-2 channels), which the reference first transforms to sRGB, give
+   MB200_EUNSUPPORTED: transform them with mb200_transform_colorspace_layout_dev first. */
+MB200_API int mb200_range_threshold_image_dev(float *buf, size_t width, size_t height, int channels, double low_black,
+    double low_white, double high_white, double high_black, int per_channel, unsigned update_mask, void *stream);
+/* PerceptibleImage (:2092), in place: PerceptibleThreshold (:2080) on the channels of `update_mask`.  Bit exact. */
+MB200_API int mb200_perceptible_image_dev(float *buf, size_t width, size_t height, int channels, double epsilon,
+    unsigned update_mask, void *stream);
 
 /* In-place point operators of MagickCore/enhance.c and statistic.c (the reference's in-place accelerate hooks,
    accelerate-private.h:50-60), on `buf`.  Gray images (1 or 2 channels) give R, G and B the gray sample; where the three
@@ -742,6 +774,14 @@ MB200_API int mb200_black_threshold_image(float *buf, size_t width, size_t heigh
 MB200_API int mb200_white_threshold_image(float *buf, size_t width, size_t height, int channels,
     int colorspace, const char *thresholds);
 MB200_API int mb200_clamp_image(float *buf, size_t width, size_t height, int channels);
+MB200_API int mb200_adaptive_threshold_image(const float *src, float *dst, size_t width, size_t height, int channels,
+    size_t window_width, size_t window_height, double bias, unsigned update_mask);
+MB200_API int mb200_auto_threshold_image(float *buf, size_t width, size_t height, int channels, int method,
+    double *threshold_percent);
+MB200_API int mb200_range_threshold_image(float *buf, size_t width, size_t height, int channels, double low_black,
+    double low_white, double high_white, double high_black, int per_channel, unsigned update_mask);
+MB200_API int mb200_perceptible_image(float *buf, size_t width, size_t height, int channels, double epsilon,
+    unsigned update_mask);
 MB200_API int mb200_contrast_image(float *buf, size_t width, size_t height, int channels, int sharpen);
 MB200_API int mb200_modulate_image(float *buf, size_t width, size_t height, int channels, double percent_brightness,
     double percent_saturation, double percent_hue, int colorspace, int illuminant);

@@ -1,12 +1,13 @@
 """Developer micro-benchmark: device-resident timings of the hot-path operators (CUDA events).
 usage: python tools/devbench.py [blur|resize|lab|dilate|erode|gauss|conv2d|stencils|hooks|enhance|layout|level|direct|distort|
-                                 geometry|all]
+                                 geometry|threshold|all]
        [size] [ref]   (ref: distort also times the reference's all-core DistortImage / RotateImage, minutes at 8192^2)"""
 import sys
 from pathlib import Path
 sys.path.insert(0, str(Path(__file__).resolve().parent.parent))
 import torch
 import imagemagick_b200 as im
+from imagemagick_b200 import _lib
 
 which = sys.argv[1] if len(sys.argv) > 1 else "all"
 size = int(sys.argv[2]) if len(sys.argv) > 2 else 8192
@@ -319,3 +320,65 @@ if which in ("geometry", "all"):
         print(f"{name:26s} {ms:9.3f} ms  {npix * 32 / ms / 1e6:8.1f} GB/s  floor {floor:6.3f} ms = {floor / ms * 100:5.1f}%",
               flush=True)
     del x, src
+
+if which in ("threshold", "all"):
+    # AdaptiveThreshold, AutoThreshold, RangeThreshold and Perceptible at size^2 RGBA, device-resident, with the card, its
+    # power limit and max SM clock.  AdaptiveThreshold is bound by its serial chains (h+1 dependent DADDs per pixel and
+    # chain, size * 4 chains), not by HBM: the time per dependent step is printed.  The in-place operators are timed on a
+    # fresh copy of the source each run; the copy is timed alone and taken off ("operator" column).  With `ref` the
+    # reference's all-core time of the same call on the same image is printed beside it (one run each).
+    import ctypes
+    import subprocess
+    import time
+    import numpy as np
+    try:
+        q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader", "-i",
+                            str(torch.cuda.current_device())], capture_output=True, text=True, timeout=30).stdout.strip()
+    except (OSError, subprocess.SubprocessError):
+        q = "unknown"
+    print(f"threshold operators on {torch.cuda.get_device_name()} (power limit, max SM clock: {q or 'unknown'})", flush=True)
+    with_ref = len(sys.argv) > 3 and sys.argv[3] == "ref"
+    ref_so = Path(__file__).resolve().parent.parent / "oracle" / "_ref" / "libmagickref_threshold.so"
+    ref = ctypes.CDLL(str(ref_so)) if with_ref and ref_so.exists() else None
+    if with_ref and ref is None:
+        print("reference not built (oracle/_ref/libmagickref_threshold.so): no reference times", flush=True)
+    src = torch.rand(size, size, 4, device="cuda") * 65535
+    x = im.Image(src)
+    work = im.Image(src.clone())
+    host = src.cpu().numpy() if ref is not None else None
+
+    def ref_ms(op, args):
+        if ref is None:
+            return ""
+        buf = np.empty(size * size * 4, np.float32)
+        buf[:] = host.reshape(-1)
+        a = (ctypes.c_double * 4)(*(list(args) + [0.0] * (4 - len(args))))
+        prop = ctypes.create_string_buffer(64)
+        t0 = time.perf_counter()
+        rc = ref.ref_threshold_op(ctypes.c_void_p(buf.ctypes.data), ctypes.c_size_t(size), ctypes.c_size_t(size), 4, op, a,
+                                  ctypes.c_long(-1), prop)
+        return f"  reference all cores {(time.perf_counter() - t0) * 1e3:10.1f} ms (rc {rc})"
+
+    def fresh(fn):
+        def run():
+            work.pixels.copy_(src)
+            fn()
+        return run
+    copy_ms = timeit(lambda: work.pixels.copy_(src), iters=9, warm=2)
+    print(f"{'device copy of the image':40s} {copy_ms:9.3f} ms", flush=True)
+    for ww in (15, 51):
+        for direct in (0, 1):
+            _lib.load().mb200_set_option(b"no_adaptive_tile", direct)
+            ms = timeit(lambda: im.AdaptiveThresholdImage(x, ww, ww, 65535 * 0.05), iters=7, warm=2)
+            fam = "direct" if direct else "auto"
+            line = (f"{'AdaptiveThreshold %dx%d+5%% (%s)' % (ww, ww, fam):40s} {ms:9.3f} ms  "
+                    f"{ms * 1e6 / (size * (ww + 1)):8.3f} ns per dependent step")
+            print(line + (ref_ms(0, (ww, ww, 65535 * 0.05)) if not direct else ""), flush=True)
+        _lib.load().mb200_set_option(b"no_adaptive_tile", 0)
+    for name, op, args, fn in [
+            ("AutoThreshold OTSU", 1, (2,), lambda: im.AutoThresholdImage(work, im.OTSUThresholdMethod)),
+            ("RangeThreshold", 2, (10000, 20000, 40000, 50000), lambda: im.RangeThresholdImage(work, 10000, 20000, 40000, 50000)),
+            ("Perceptible 1000", 3, (1000.0,), lambda: im.PerceptibleImage(work, 1000.0))]:
+        ms = timeit(fresh(fn), iters=9, warm=2)
+        print(f"{name:40s} copy + operator {ms:9.3f} ms  operator {ms - copy_ms:7.3f} ms" + ref_ms(op, args), flush=True)
+    del x, work, src
