@@ -92,6 +92,10 @@ PROTOTYPES = {
     "mb200_geometry_plan": (_i, [_i, _sz, _sz, _vp, _vp, _vp]),
     "mb200_geometry_image_dev": (_i, [_vp, _sz, _sz, _i, _vp, _vp, _vp]),
     "mb200_geometry_image": (_i, [_vp, _sz, _sz, _i, _vp, _vp]),
+    "mb200_bounding_box_from_rows": (_i, [_vp, _sz, _sz, _i, _vp, _vp]),
+    "mb200_trim_plan": (_i, [_sz, _sz, _vp, _vp, _i, _vp, _vp]),
+    "mb200_bounding_box_dev": (_i, [_vp, _sz, _sz, _i, _vp, _vp, _vp, _vp]),
+    "mb200_bounding_box": (_i, [_vp, _sz, _sz, _i, _vp, _vp, _vp]),
     "mb200_resample_filter_lut": (_i, [_i, _vp, _vp, _vp]),
     "mb200_convolve_image_dev": (_i, [_vp, _vp, _sz, _sz, _i, KernelPtr, _vp]),
     "mb200_blur_image_dev": (_i, [_vp, _vp, _sz, _sz, _i, _d, _d, _vp]),

@@ -26,6 +26,7 @@ include/magick_b200.h:
     CropImage, ShaveImage, RollImage, AutoOrientImage               transform.c:542/1641/1546/103
     FlipImage, FlopImage, TransposeImage, TransverseImage           transform.c:1194/1329/2127/2265
     IntegralRotateImage                                             shear.c:700
+    GetImageBoundingBox, TrimImage                                  attribute.c:391, transform.c:2412
 
 An `Image` wraps the pixel cache: an (rows, columns, channels) float32 array of raw
 Quantum values (0..65535), either a NumPy array (host; every call stages through
@@ -538,7 +539,10 @@ def GeometryPlan(image: Image, op: int, arguments=()) -> GeometryParams:
 
 
 def _geometry(image: Image, op: int, arguments=()) -> Image:
-    plan = GeometryPlan(image, op, arguments)
+    return _run_geometry(image, GeometryPlan(image, op, arguments))
+
+
+def _run_geometry(image: Image, plan: GeometryParams) -> Image:
     lib = _lib.load()
     out = image._new_like(rows=plan.rows, columns=plan.columns)
     if image.on_device:
@@ -607,6 +611,72 @@ def AutoOrientImage(image: Image, orientation: int) -> Image:
     if orientation not in ops:
         raise MagickB200Error(_lib.EUNSUPPORTED, "auto-orient: already TopLeft (the reference returns a clone)")
     return _geometry(image, *ops[orientation])
+
+
+# MagickCore/geometry.h GravityType
+(UndefinedGravity, NorthWestGravity, NorthGravity, NorthEastGravity, WestGravity, CenterGravity, EastGravity,
+ SouthWestGravity, SouthGravity, SouthEastGravity) = range(10)
+ForgetGravity = UndefinedGravity
+# mb200_trim_edge: the edges a "trim:edges" artifact names
+TrimEdgeNorth, TrimEdgeEast, TrimEdgeSouth, TrimEdgeWest = 1, 2, 4, 8
+TRIM_EDGES_UNSET = -1
+
+
+class TrimOptions(C.Structure):
+    """mb200_trim_options: the image settings GetImageBoundingBox reads."""
+    _fields_ = [("fuzz", C.c_double), ("edges", C.c_int), ("colorspace", C.c_int)]
+
+
+def trim_edges(artifact: Optional[str]) -> int:
+    """The mb200_trim_edge bits of a "trim:edges" artifact, split on ',' and compared without case as attribute.c:444-454
+    does (other tokens count for nothing); TRIM_EDGES_UNSET for None."""
+    if artifact is None:
+        return TRIM_EDGES_UNSET
+    bits = {"north": TrimEdgeNorth, "east": TrimEdgeEast, "south": TrimEdgeSouth, "west": TrimEdgeWest}
+    edges = 0
+    for token in artifact.split(","):
+        edges |= bits.get(token.lower(), 0)
+    return edges
+
+
+def BoundingBoxWarning(image: Image, fuzz: float = 0.0, edges: Optional[str] = None):
+    """GetImageBoundingBox's box and whether the reference warns GeometryDoesNotContainImage for it (the scan left a
+    zero width or height; the final arithmetic can give a zero side without the warning)."""
+    options = TrimOptions(float(fuzz), trim_edges(edges), int(image.colorspace))
+    box = Page()
+    warning = C.c_int(0)
+    lib = _lib.load()
+    if image.on_device:
+        _activate(image)
+        check(lib.mb200_bounding_box_dev(image._ptr(), image.columns, image.rows, image.channels, C.byref(options),
+                                         C.byref(box), C.byref(warning), _stream(image)))
+    else:
+        check(lib.mb200_bounding_box(image._ptr(), image.columns, image.rows, image.channels, C.byref(options),
+                                     C.byref(box), C.byref(warning)))
+    return (int(box.width), int(box.height), int(box.x), int(box.y)), bool(warning.value)
+
+
+def GetImageBoundingBox(image: Image, fuzz: float = 0.0, edges: Optional[str] = None):
+    """MagickCore/attribute.c:391 -- (width, height, x, y) of the region that differs, beyond `fuzz`, from the corner
+    pixels; `edges` is the "trim:edges" artifact.  Bit exact, with the reference's single-threaded result.  A box of zero
+    width or height is returned as it is (BoundingBoxWarning tells whether the reference warns)."""
+    return BoundingBoxWarning(image, fuzz, edges)[0]
+
+
+def TrimImage(image: Image, fuzz: float = 0.0, edges: Optional[str] = None, min_size=None,
+              gravity: int = UndefinedGravity) -> Image:
+    """MagickCore/transform.c:2412: CropImage to GetImageBoundingBox, grown to `min_size` (width, height; the
+    "trim:minSize" artifact) under `gravity` when both sides of the box are smaller.  Bit exact; one bounding-box scan
+    and one crop.  A zero box raises MB200_EUNSUPPORTED (the reference warns and returns a transparent 1x1 image), as do
+    the crops CropImage declines."""
+    width, height, x, y = GetImageBoundingBox(image, fuzz, edges)
+    box = Page(width, height, x, y)
+    page = Page(*image.page_size, *image.page)
+    size = None if min_size is None else (C.c_size_t * 2)(*[int(v) for v in min_size])
+    plan = GeometryParams()
+    check(_lib.load().mb200_trim_plan(image.columns, image.rows, C.byref(page), C.byref(box), int(gravity), size,
+                                      C.byref(plan)))
+    return _run_geometry(image, plan)
 
 
 def SampleImage(image: Image, columns: int, rows: int) -> Image:

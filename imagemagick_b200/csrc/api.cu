@@ -489,6 +489,31 @@ int mb200_geometry_image_dev(const float *src, size_t width, size_t height, int 
   return launch_geometry(src, width, height, channels, dst, plan, s);
 }
 
+// The scan writes the row summaries into a pool temporary; they come back to the host for the serial rule.
+int mb200_bounding_box_dev(const float *src, size_t width, size_t height, int channels,
+                           const mb200_trim_options *options, mb200_page *box, int *warning, void *stream) {
+  if (!src || !box) return fail(MB200_EINVAL, "bounding box: bad arguments");
+  int rc = bounding_box_check(width, height, channels, options);
+  cudaStream_t s;
+  if (!rc) rc = prepare(stream, &s);
+  if (rc) return rc;
+  std::vector<unsigned> summaries(height * 4);
+  {
+    StreamAlloc rows(s);
+    rc = rows.alloc(summaries.size() * sizeof(unsigned));
+    if (!rc) rc = launch_bounding_box(src, width, height, channels, options, static_cast<unsigned *>(rows.ptr), s);
+    if (!rc) {
+      const cudaError_t e = cudaMemcpyAsync(summaries.data(), rows.ptr, summaries.size() * sizeof(unsigned),
+                                            cudaMemcpyDeviceToHost, s);
+      if (e != cudaSuccess) rc = cuda_fail(e, "bounding box: summaries");
+    }
+  }
+  const cudaError_t e = cudaStreamSynchronize(s);
+  if (!rc && e != cudaSuccess) rc = cuda_fail(e, "bounding box");
+  if (rc) return rc;
+  return mb200_bounding_box_from_rows(summaries.data(), width, height, options->edges, box, warning);
+}
+
 int mb200_convolve_image_dev(const float *src, float *dst, size_t width, size_t height, int channels,
                              const mb200_kernel_info *kernel, void *stream) {
   return mb200_morphology_image_dev(src, dst, width, height, channels, MB200_ConvolveMorphology, 1, kernel, 0.0,
@@ -687,6 +712,21 @@ int mb200_geometry_image(const float *src, size_t w, size_t h, int ch, float *ds
                       [&](const float *s, float *d, cudaStream_t st) {
     return mb200_geometry_image_dev(s, w, h, ch, d, plan, st);
   });
+}
+
+int mb200_bounding_box(const float *src, size_t w, size_t h, int ch, const mb200_trim_options *options,
+                       mb200_page *box, int *warning) {
+  if (!src || !box) return fail(MB200_EINVAL, "bounding box: bad arguments");
+  int rc = bounding_box_check(w, h, ch, options);
+  cudaStream_t s;
+  if (!rc) rc = prepare(nullptr, &s);
+  if (rc) return rc;
+  StageRef in;                                                   // read only: nothing is copied back
+  rc = stage_input(src, image_bytes(w, h, ch), s, &in);
+  if (!rc) rc = mb200_bounding_box_dev(static_cast<const float *>(in.dev), w, h, ch, options, box, warning, s);
+  if (rc) cudaStreamSynchronize(s);
+  release_stage(&in, s);
+  return rc;
 }
 
 int mb200_unsharp_mask_image(const float *src, float *dst, size_t w, size_t h, int ch, double radius, double sigma,

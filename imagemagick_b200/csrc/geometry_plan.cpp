@@ -4,8 +4,9 @@
 // Behavioural mirror of MagickCore/transform.c: CropImage's bounding box, clamps and page rule (:580-677), ShaveImage's
 // geometry (:1654-1668), the page updates of FlipImage (:1294-1298), FlopImage (:1430-1434), TransposeImage
 // (:2230-2234) and TransverseImage (:2372-2380), RollImage's offset normalisation (:1572-1581); and shear.c's
-// IntegralRotateImage (rotations mod 4, the page swaps :1060-1092).  size_t / ssize_t arithmetic is the reference's,
-// wrap-around included.  No device.
+// IntegralRotateImage (rotations mod 4, the page swaps :1060-1092).  Also the host half of GetImageBoundingBox
+// (attribute.c:487-560, the serial rule over trim.cu's row summaries) and TrimImage's geometry (transform.c:2445-2509).
+// size_t / ssize_t arithmetic is the reference's, wrap-around included.  No device.
 #include "mb200_internal.h"
 
 #include <cmath>
@@ -207,6 +208,92 @@ int mb200_geometry_plan(int op, size_t columns, size_t rows, const mb200_page *p
   }
   *plan = p;
   return MB200_OK;
+}
+
+// GetImageBoundingBox's row loop (attribute.c:487-551) run on the row summaries, in the single-threaded order.  Row y
+// starts from the bounds the rows before it left, and its updates reduce as follows:
+//   - x: the first x that mismatches target 0, when it is below the bounds' x (:517-519);
+//   - y: y itself, when some x mismatches target 0 and y is below the bounds' y (:523-525);
+//   - width: the last x that mismatches target 1, when it is above the width W the row started with (:520-522).  The
+//     target 3 rule (:529-535) can lower the row's width, but only to an x below W, and the merge (:546) keeps the
+//     larger of W and the row's width, so a lowered width never survives;
+//   - height: y, when y is above the height the row started with and either some x mismatches target 2 (:526-528) or
+//     the target 3 rule fires.  That rule fires at most once per row (it sets the height to y), at the first x that
+//     mismatches target 3, and only if that x is below W: a target 1 update raises the width to some x' > W, and every
+//     later x is above x'.
+// Each row reads only the bounds the rows above it left, so the serial order is one pass over the rows.
+int mb200_bounding_box_from_rows(const unsigned *summaries, size_t columns, size_t rows, int edges, mb200_page *box,
+                                 int *warning) {
+  if (!summaries || !box || columns == 0 || rows == 0 || edges < MB200_TRIM_EDGES_UNSET || edges > 15)
+    return mb200::fail(MB200_EINVAL, "bounding box: bad arguments");
+  const long cols = static_cast<long>(columns), nrows = static_cast<long>(rows);
+  long x, y, width, height;                                                  // :423-456
+  if (edges == MB200_TRIM_EDGES_UNSET) {
+    width = columns == 1 ? 1 : 0;
+    height = rows == 1 ? 1 : 0;
+    x = cols;
+    y = nrows;
+  } else {
+    width = cols;
+    height = nrows;
+    x = 0;
+    y = 0;
+    if (edges & MB200_TrimEdgeNorth) y = nrows;
+    if (edges & MB200_TrimEdgeEast) width = 0;
+    if (edges & MB200_TrimEdgeSouth) height = 0;
+    if (edges & MB200_TrimEdgeWest) x = cols;
+  }
+  for (long r = 0; r < nrows; ++r) {
+    const unsigned *s = summaries + 4 * r;
+    const long first0 = s[0] ? cols - static_cast<long>(s[0]) : cols;
+    const long last1 = static_cast<long>(s[1]) - 1;
+    const long first3 = s[3] ? cols - static_cast<long>(s[3]) : cols;
+    if (first0 < x) x = first0;
+    if (first0 < cols && r < y) y = r;
+    if (r > height && (s[2] != 0 || first3 < width)) height = r;
+    if (last1 > width) width = last1;
+  }
+  box->x = x;
+  box->y = y;
+  box->width = static_cast<size_t>(width);
+  box->height = static_cast<size_t>(height);
+  const bool empty = box->width == 0 || box->height == 0;                    // :553-560
+  if (!empty) {
+    box->width -= static_cast<size_t>(x - 1);
+    box->height -= static_cast<size_t>(y - 1);
+  }
+  if (warning) *warning = empty ? 1 : 0;
+  return MB200_OK;
+}
+
+int mb200_trim_plan(size_t columns, size_t rows, const mb200_page *page, const mb200_page *box, int gravity,
+                    const size_t *min_size, mb200_geometry_params *plan) {
+  if (!page || !box || !plan || gravity < MB200_UndefinedGravity || gravity > MB200_SouthEastGravity)
+    return mb200::fail(MB200_EINVAL, "trim plan: bad arguments");
+  if (box->width == 0 || box->height == 0)                                   // transform.c:2429-2444
+    return mb200::fail(MB200_EUNSUPPORTED, "trim: GeometryDoesNotContainImage (the reference returns a 1x1 clone)");
+  mb200_page geometry = *box;
+  if (min_size && geometry.width < min_size[0] && geometry.height < min_size[1]) {   // :2445-2507
+    const long dw = static_cast<long>(min_size[0]) - static_cast<long>(geometry.width);
+    const long dh = static_cast<long>(min_size[1]) - static_cast<long>(geometry.height);
+    switch (gravity) {
+      case MB200_CenterGravity: geometry.x -= dw / 2; geometry.y -= dh / 2; break;
+      case MB200_NorthWestGravity: geometry.x -= dw; geometry.y -= dh; break;
+      case MB200_NorthGravity: geometry.x -= dw / 2; geometry.y -= dh; break;
+      case MB200_NorthEastGravity: geometry.y -= dh; break;
+      case MB200_EastGravity: geometry.y -= dh / 2; break;
+      case MB200_SouthGravity: geometry.x -= dw / 2; break;
+      case MB200_SouthWestGravity: geometry.x -= dw; break;
+      case MB200_WestGravity: geometry.x -= dw; geometry.y -= dh / 2; break;
+      default: break;                                                        // SouthEast, Undefined
+    }
+    geometry.width = min_size[0];
+    geometry.height = min_size[1];
+  }
+  geometry.x += page->x;                                                     // :2508-2510
+  geometry.y += page->y;
+  const long args[4] = {static_cast<long>(geometry.width), static_cast<long>(geometry.height), geometry.x, geometry.y};
+  return mb200_geometry_plan(MB200_GeometryCrop, columns, rows, page, args, plan);
 }
 
 }  // extern "C"

@@ -46,6 +46,7 @@ enum LaunchFamily {
   kDistort,                                                            // distort.cu
   kGeometry,                                                           // geometry.cu
   kAdaptiveThresholdTile, kAdaptiveThresholdDirect,                    // threshold.cu
+  kBoundingBox,                                                        // trim.cu
   kLaunchFamilies
 };
 void count_family(LaunchFamily family);
@@ -144,6 +145,12 @@ int launch_distort(const float *src, size_t width, size_t height, int channels, 
 int geometry_check(size_t width, size_t height, int channels, const mb200_geometry_params *plan);
 int launch_geometry(const float *src, size_t width, size_t height, int channels, float *dst,
                     const mb200_geometry_params *plan, void *stream);
+
+// trim.cu: GetImageBoundingBox's scan into d_rows (height x 4 words, the format of mb200_bounding_box_from_rows).  The
+// check runs on the host before anything is touched; the launch is one memset and one kernel.
+int bounding_box_check(size_t width, size_t height, int channels, const mb200_trim_options *options);
+int launch_bounding_box(const float *src, size_t width, size_t height, int channels, const mb200_trim_options *options,
+                        unsigned *d_rows, void *stream);
 
 // ---- resize axis tables (resize_tables.cpp) ---------------------------------
 // One axis of ResizeImage, planned on the host and resident on one device: the reference's contribution lists

@@ -145,7 +145,8 @@ const char *const kFamilyNames[kLaunchFamilies] = {
     "resize_v_stream_launches", "resize_h_tma_launches", "resize_h_stream_launches", "resize_fused_launches",
     "resize_regular_launches", "resize_gather_launches", "conv2d_dense_r8_launches", "conv2d_dense_r4_launches",
     "conv2d_dense_r2_launches", "morph2d_launches", "minmax2d_launches", "morph_stream_launches", "morph_direct_launches",
-    "distort_launches", "geometry_launches", "adaptive_threshold_tile_launches", "adaptive_threshold_direct_launches"};
+    "distort_launches", "geometry_launches", "adaptive_threshold_tile_launches", "adaptive_threshold_direct_launches",
+    "bounding_box_launches"};
 std::atomic<unsigned long long> g_family_launches[kLaunchFamilies];
 int family_index(const char *name) {
   for (int f = 0; f < kLaunchFamilies; ++f)

@@ -1735,11 +1735,12 @@ Image *__wrap_RotateImage(const Image *image, const double degrees, ExceptionInf
    NULL == declined, with the caller's exception untouched: no device, a layout the library does not take (CMYK,
    PseudoClass, masks, meta channels), and the plan's declines (a crop outside the canvas or of zero area, a shave of
    half the image, IntegralRotateImage by 0). */
+static Image *b200_run_geometry(const Image *image, int ch, const mb200_geometry_params *p);
+
 static Image *b200_geometry(const Image *image, int op, const long *args)
 {
   mb200_geometry_params plan;
   mb200_page page;
-  Image *out = (Image *) NULL;
   int ch;
   if (mb200_device_count() <= 0) return (Image *) NULL;
   ch = b200_layout_masked(image, (unsigned *) NULL);
@@ -1747,6 +1748,14 @@ static Image *b200_geometry(const Image *image, int op, const long *args)
   page.width = image->page.width; page.height = image->page.height; page.x = (long) image->page.x;
   page.y = (long) image->page.y;
   if (mb200_geometry_plan(op, image->columns, image->rows, &page, args, &plan) != MB200_OK) return (Image *) NULL;
+  return b200_run_geometry(image, ch, &plan);
+}
+
+/* A plan of mb200_geometry_plan (or mb200_trim_plan) on an image of `ch` channels: the result image, or NULL. */
+static Image *b200_run_geometry(const Image *image, int ch, const mb200_geometry_params *p)
+{
+  const mb200_geometry_params plan = *p;
+  Image *out = (Image *) NULL;
   {
     B200_ATTEMPT_BEGIN;
     const float *p = b200_cache_pixels(image, ch, attempt);
@@ -1919,6 +1928,121 @@ Image *__wrap_AutoOrientImage(const Image *image, const OrientationType orientat
 {
   TRY(b200_auto_orient(image, orientation));
   return __real_AutoOrientImage(image, orientation, exception);
+}
+
+/* ---- GetImageBoundingBox (attribute.c:391) and TrimImage (transform.c:2412) --------------------------------------------
+   The box is mb200_bounding_box on the pixel cache, with the image's fuzz, "trim:edges" (split and compared with the
+   reference's own StringToken / LocaleCompare) and colourspace.  TrimImage needs a wrap of its own: its call to CropImage
+   stays inside transform.o (its call to GetImageBoundingBox crosses objects).  Declined, with the caller's exception
+   untouched: no device, a layout the library does not take (CMYK, PseudoClass, masks, meta channels), and
+   "trim:percent-background" (GetEdgeBoundingBox, another algorithm); TrimImage also declines an image with an 8bim
+   profile (Update8BIMClipPath rewrites its clip path) and the crops mb200_trim_plan declines. */
+static int b200_bounding_box(const Image *image, RectangleInfo *box, int *warning)
+{
+  mb200_trim_options options;
+  mb200_page b;
+  const char *edges;
+  int ch, rc = MB200_EUNSUPPORTED;
+  if (mb200_device_count() <= 0 || GetImageArtifact(image, "trim:percent-background") != (const char *) NULL) return 0;
+  ch = b200_layout_masked(image, (unsigned *) NULL);
+  if (ch == 0) return 0;
+  options.fuzz = image->fuzz;
+  options.colorspace = (int) image->colorspace;
+  options.edges = MB200_TRIM_EDGES_UNSET;
+  edges = GetImageArtifact(image, "trim:edges");
+  if (edges != (const char *) NULL) {                                        /* attribute.c:442-455 */
+    char *copy = AcquireString(edges), *r = copy, *q;
+    options.edges = 0;
+    while ((q = StringToken(",", &r)) != (char *) NULL) {
+      if (LocaleCompare(q, "north") == 0) options.edges |= MB200_TrimEdgeNorth;
+      if (LocaleCompare(q, "east") == 0) options.edges |= MB200_TrimEdgeEast;
+      if (LocaleCompare(q, "south") == 0) options.edges |= MB200_TrimEdgeSouth;
+      if (LocaleCompare(q, "west") == 0) options.edges |= MB200_TrimEdgeWest;
+    }
+    copy = DestroyString(copy);
+  }
+  {
+    B200_ATTEMPT_BEGIN;
+    const float *p = b200_cache_pixels(image, ch, attempt);
+    if (p != (const float *) NULL) rc = mb200_bounding_box(p, image->columns, image->rows, ch, &options, &b, warning);
+    B200_ATTEMPT_END;
+  }
+  if (rc != MB200_OK) return 0;
+  box->width = b.width; box->height = b.height; box->x = (ssize_t) b.x; box->y = (ssize_t) b.y;
+  return 1;
+}
+
+static void b200_box_warning(const Image *image, ExceptionInfo *exception)      /* attribute.c:553-555 */
+{
+  (void) ThrowMagickException(exception, GetMagickModule(), OptionWarning, "GeometryDoesNotContainImage", "`%s'",
+                              image->filename);
+}
+
+extern RectangleInfo __real_GetImageBoundingBox(const Image *, ExceptionInfo *);
+extern Image *__real_TrimImage(const Image *, ExceptionInfo *);
+
+RectangleInfo __wrap_GetImageBoundingBox(const Image *image, ExceptionInfo *exception)
+{
+  if (b200_on()) {
+    RectangleInfo box;
+    int warning = 0;
+    if (b200_bounding_box(image, &box, &warning)) {
+      B200_COUNT(b200_hits);
+      if (warning) b200_box_warning(image, exception);
+      return box;
+    }
+    B200_COUNT(b200_fallbacks);
+  }
+  return __real_GetImageBoundingBox(image, exception);
+}
+
+Image *__wrap_TrimImage(const Image *image, ExceptionInfo *exception)
+{
+  if (b200_on()) {
+    RectangleInfo box;
+    int warning = 0;
+    const int ch = b200_layout_masked(image, (unsigned *) NULL);
+    if (ch != 0 && GetImageProfile(image, "8bim") == (const StringInfo *) NULL &&
+        b200_bounding_box(image, &box, &warning)) {
+      Image *out = (Image *) NULL;
+      if (box.width == 0 || box.height == 0) {                               /* transform.c:2429-2444, no pixel read */
+        B200_COUNT(b200_hits);
+        if (warning) b200_box_warning(image, exception);
+        out = CloneImage(image, 1, 1, MagickTrue, exception);
+        if (out == (Image *) NULL) return out;
+        out->background_color.alpha_trait = BlendPixelTrait;
+        out->background_color.alpha = (MagickRealType) TransparentAlpha;
+        (void) SetImageBackgroundColor(out, exception);
+        out->page = image->page;
+        out->page.x = -1;
+        out->page.y = -1;
+        return out;
+      }
+      {
+        mb200_geometry_params plan;
+        mb200_page page, b;
+        size_t min_size[2];
+        const char *artifact = GetImageArtifact(image, "trim:minSize");
+        page.width = image->page.width; page.height = image->page.height;
+        page.x = (long) image->page.x; page.y = (long) image->page.y;
+        b.width = box.width; b.height = box.height; b.x = (long) box.x; b.y = (long) box.y;
+        if (artifact != (const char *) NULL) {                               /* :2445-2448 */
+          RectangleInfo size = box;
+          (void) ParseAbsoluteGeometry(artifact, &size);
+          min_size[0] = size.width; min_size[1] = size.height;
+        }
+        if (mb200_trim_plan(image->columns, image->rows, &page, &b, (int) image->gravity,
+                            artifact != (const char *) NULL ? min_size : (const size_t *) NULL, &plan) == MB200_OK)
+          out = b200_run_geometry(image, ch, &plan);
+      }
+      if (out != (Image *) NULL) {
+        B200_COUNT(b200_hits);
+        return out;
+      }
+    }
+    B200_COUNT(b200_fallbacks);
+  }
+  return __real_TrimImage(image, exception);
 }
 
 MagickBooleanType __wrap_NormalizeImage(Image *image, ExceptionInfo *exception)

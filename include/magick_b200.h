@@ -205,7 +205,7 @@ MB200_API int mb200_probe_fp64_fma_rate(double *fma_per_second);
    "conv_pair_launches", "conv_pair_async_launches", "conv_generic_launches", "resize_v_stream_launches",
    "resize_h_tma_launches", "resize_h_stream_launches", "resize_fused_launches", "resize_regular_launches",
    "resize_gather_launches", "adaptive_threshold_tile_launches", "adaptive_threshold_direct_launches" (with the switch
-   "no_adaptive_tile", which sends AdaptiveThresholdImage to its direct family). */
+   "no_adaptive_tile", which sends AdaptiveThresholdImage to its direct family), "bounding_box_launches". */
 MB200_API int mb200_set_option(const char *name, int value);
 MB200_API int mb200_get_option(const char *name, int *value);
 
@@ -375,6 +375,45 @@ typedef struct mb200_geometry_params {
 MB200_API int mb200_geometry_plan(int op, size_t columns, size_t rows, const mb200_page *page, const long *args,
     mb200_geometry_params *plan);
 
+/* ---- GetImageBoundingBox (MagickCore/attribute.c:391) and TrimImage (transform.c:2412) ----
+   The image's settings the bounding box reads: its fuzz, the "trim:edges" artifact as a bitmask of the edges it names
+   (MB200_TRIM_EDGES_UNSET when the artifact is not set; 0 when it names none of the four), and its colourspace (CMYK
+   adds the black term to the fuzzy comparison and needs 4 or 5 channels, HCL / HCLp / HSB / HSI / HSL / HSV measure the
+   first channel as a hue arc, anything else compares plainly).  "trim:percent-background" selects another algorithm
+   (GetEdgeBoundingBox) that is not served here. */
+typedef enum {
+  MB200_TrimEdgeNorth = 1, MB200_TrimEdgeEast = 2, MB200_TrimEdgeSouth = 4, MB200_TrimEdgeWest = 8
+} mb200_trim_edge;
+#define MB200_TRIM_EDGES_UNSET (-1)
+typedef struct mb200_trim_options {
+  double fuzz;                   /* image->fuzz, in quantum units */
+  int edges;                     /* mb200_trim_edge bits, or MB200_TRIM_EDGES_UNSET */
+  int colorspace;                /* mb200_colorspace */
+} mb200_trim_options;
+/* MagickCore/geometry.h GravityType -- same numeric values */
+typedef enum {
+  MB200_UndefinedGravity = 0, MB200_NorthWestGravity = 1, MB200_NorthGravity = 2, MB200_NorthEastGravity = 3,
+  MB200_WestGravity = 4, MB200_CenterGravity = 5, MB200_EastGravity = 6, MB200_SouthWestGravity = 7,
+  MB200_SouthGravity = 8, MB200_SouthEastGravity = 9
+} mb200_gravity;
+/* The host half of GetImageBoundingBox, without a device.  `summaries` holds 4 words per row, all 0 when nothing in the
+   row mismatches: [0] columns - the first x not fuzzy-equivalent to the top-left pixel, [1] 1 + the last x not
+   equivalent to the top-right pixel, [2] nonzero when any x is not equivalent to the bottom-left pixel, [3] columns -
+   the first x not equivalent to the bottom-right pixel.  *box receives what the reference's single-threaded row loop
+   (:487-551) computes from the initial bounds `edges` gives, after its final arithmetic (:553-560, in size_t, so a
+   one-column image can give width 2).  *warning (may be NULL) is set to 1 where the reference warns
+   "GeometryDoesNotContainImage" -- the loop left a zero width or height, and the box is returned as it is -- and to 0
+   otherwise: the final arithmetic can itself give a zero side, without the warning.  MB200_EINVAL: no buffer, an empty
+   image, a bad `edges`. */
+MB200_API int mb200_bounding_box_from_rows(const unsigned *summaries, size_t columns, size_t rows, int edges,
+    mb200_page *box, int *warning);
+/* TrimImage's geometry (:2445-2509) for a bounding box `box` of a columns x rows image with page `page`: the box grown
+   to `min_size` (width, height; NULL: no "trim:minSize") under `gravity` when both of its sides are smaller, offset by
+   the page, then the CropImage plan of mb200_geometry_plan.  MB200_EUNSUPPORTED for a zero box (the reference returns a
+   transparent 1x1 clone) and wherever the crop plan declines. */
+MB200_API int mb200_trim_plan(size_t columns, size_t rows, const mb200_page *page, const mb200_page *box, int gravity,
+    const size_t *min_size, mb200_geometry_params *plan);
+
 /* --------------------------------------- device-resident operators (HBM) ---- */
 /* src/dst are DEVICE pointers (from mb200_malloc or any CUDA allocation, e.g. a
    torch tensor's data_ptr()); they must not alias unless stated.  `stream` is a
@@ -429,6 +468,15 @@ MB200_API int mb200_distort_image_dev(const float *src, size_t width, size_t hei
    MB200_EINVAL, before the device is touched: a map or source rectangle that does not fit the source image. */
 MB200_API int mb200_geometry_image_dev(const float *src, size_t width, size_t height, int channels, float *dst,
     const mb200_geometry_params *plan, void *stream);
+
+/* GetImageBoundingBox (MagickCore/attribute.c:391) of `src` (1-5 channels: gray, gray + alpha, RGB, RGBA, or CMYK and
+   CMYKA when options->colorspace is CMYK): one scan for the row summaries of mb200_bounding_box_from_rows, with
+   IsFuzzyEquivalencePixelInfo (pixel.c:6028) restated in double, then that function.  Bit exact, with the reference's
+   single-threaded result on images of any height; *warning (may be NULL) as there.  Synchronises `stream` to return
+   *box.  MB200_EINVAL, before the device is touched: bad options or a channel count the colourspace does not have;
+   MB200_EUNSUPPORTED: images wider than 2^32 - 1. */
+MB200_API int mb200_bounding_box_dev(const float *src, size_t width, size_t height, int channels,
+    const mb200_trim_options *options, mb200_page *box, int *warning, void *stream);
 
 /* ConvolveImage (MagickCore/effect.c:1170) */
 MB200_API int mb200_convolve_image_dev(const float *src, float *dst, size_t width, size_t height,
@@ -722,6 +770,8 @@ MB200_API int mb200_distort_image(const float *src, size_t width, size_t height,
     const mb200_distort_params *plan, const mb200_resample_options *options);
 MB200_API int mb200_geometry_image(const float *src, size_t width, size_t height, int channels, float *dst,
     const mb200_geometry_params *plan);
+MB200_API int mb200_bounding_box(const float *src, size_t width, size_t height, int channels,
+    const mb200_trim_options *options, mb200_page *box, int *warning);
 MB200_API int mb200_sharpen_image(const float *src, float *dst, size_t width, size_t height, int channels,
     double radius, double sigma);
 MB200_API int mb200_edge_image(const float *src, float *dst, size_t width, size_t height, int channels,

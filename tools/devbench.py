@@ -1,7 +1,8 @@
 """Developer micro-benchmark: device-resident timings of the hot-path operators (CUDA events).
 usage: python tools/devbench.py [blur|resize|lab|dilate|erode|gauss|conv2d|stencils|hooks|enhance|layout|level|direct|distort|
-                                 geometry|threshold|all]
-       [size] [ref]   (ref: distort also times the reference's all-core DistortImage / RotateImage, minutes at 8192^2)"""
+                                 geometry|threshold|trim|all]
+       [size] [ref]   (ref: distort also times the reference's all-core DistortImage / RotateImage, minutes at 8192^2;
+                       threshold and trim time the reference's all-core call beside theirs)"""
 import sys
 from pathlib import Path
 sys.path.insert(0, str(Path(__file__).resolve().parent.parent))
@@ -382,3 +383,66 @@ if which in ("threshold", "all"):
         ms = timeit(fresh(fn), iters=9, warm=2)
         print(f"{name:40s} copy + operator {ms:9.3f} ms  operator {ms - copy_ms:7.3f} ms" + ref_ms(op, args), flush=True)
     del x, work, src
+
+if which in ("trim", "all"):
+    # GetImageBoundingBox and TrimImage at size^2 RGBA, device-resident, with the card, its power limit and max SM clock:
+    # a framed object on a background whose four corners are equal (one comparison per pixel), then four distinct
+    # corners (four).  The box call includes its readback of size * 16 B of row summaries and the synchronise.  Floors:
+    # 16 B/px read at the 3.35 TB/s H100 SXM data-sheet HBM bandwidth, and the FP64 pipe at its data-sheet 33.5 TFLOP/s
+    # (one operation per FP64 instruction: 64 per SM and clock) for the comparisons' FP64 instructions, counted from
+    # fuzzy.cuh for RGBA: 4 float -> double conversions per pixel, and per comparison 6 for the alpha term, 1 for the x3
+    # rescale and 5 per colour term (sub, mul, mul, add, compare) = 22.  With `ref` the reference's all-core time of the
+    # same call on the same image is printed beside it (one run each).
+    import ctypes
+    import os
+    import subprocess
+    import time
+    import numpy as np
+    DATASHEET_BW, DATASHEET_FP64 = 3350.0, 33.5e12
+    try:
+        q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader", "-i",
+                            str(torch.cuda.current_device())], capture_output=True, text=True, timeout=30).stdout.strip()
+    except (OSError, subprocess.SubprocessError):
+        q = "unknown"
+    print(f"bounding box and trim on {torch.cuda.get_device_name()} (power limit, max SM clock: {q or 'unknown'})",
+          flush=True)
+    with_ref = len(sys.argv) > 3 and sys.argv[3] == "ref"
+    ref_so = Path(__file__).resolve().parent.parent / "oracle" / "_ref" / "libmagickref_trim.so"
+    ref = ctypes.CDLL(str(ref_so)) if with_ref and ref_so.exists() else None
+    if with_ref and ref is None:
+        print("reference not built (oracle/_ref/libmagickref_trim.so): no reference times", flush=True)
+    src = torch.full((size, size, 4), 1000.0, device="cuda")
+    src[..., 1] = 20000.0
+    src[..., 3] = 65535.0
+    src[size // 5: size - size // 4, size // 6: size - size // 3] = torch.rand(size - size // 4 - size // 5,
+                                                                               size - size // 3 - size // 6, 4,
+                                                                               device="cuda") * 65535
+    floor_bw = size * size * 16 / DATASHEET_BW / 1e6
+
+    def ref_ms(image, op):
+        if ref is None:
+            return ""
+        host = np.ascontiguousarray(image.cpu().numpy())
+        lp = ctypes.c_long * 7
+        box, geom, sev = lp(), lp(), ctypes.c_int(0)
+        out = np.empty(host.size, np.float32) if op == 1 else np.empty(1, np.float32)
+        t0 = time.perf_counter()
+        rc = ref.ref_trim(ctypes.c_void_p(host.ctypes.data), ctypes.c_size_t(size), ctypes.c_size_t(size), 4, 0, -1,
+                          (ctypes.c_long * 4)(), ctypes.c_double(0.0), None, None, 0, op, box, ctypes.byref(sev),
+                          ctypes.c_void_p(out.ctypes.data), ctypes.c_size_t(out.size), geom, os.cpu_count())
+        return f"  reference all cores {(time.perf_counter() - t0) * 1e3:9.1f} ms (rc {rc}, {os.cpu_count()} threads)"
+
+    for corners in ("equal corners", "four distinct corners"):
+        if corners != "equal corners":
+            for k, (y, x) in enumerate([(0, 0), (0, size - 1), (size - 1, 0), (size - 1, size - 1)]):
+                src[y, x, 0] = 1000.0 + 3000.0 * k
+        x = im.Image(src)
+        compares = 1 if corners == "equal corners" else 4
+        floor_fp64 = size * size * (4 + 22 * compares) / DATASHEET_FP64 * 1e3
+        ms = timeit(lambda: im.GetImageBoundingBox(x), iters=20, warm=3)
+        print(f"{'GetImageBoundingBox ' + corners:44s} {ms:8.3f} ms  HBM floor {floor_bw:6.3f} ms ({floor_bw / ms * 100:5.1f}%)"
+              f"  FP64 floor {floor_fp64:6.3f} ms ({floor_fp64 / ms * 100:5.1f}%)  box {im.GetImageBoundingBox(x)}"
+              + ref_ms(src, 0), flush=True)
+        ms = timeit(lambda: im.TrimImage(x), iters=20, warm=3)
+        print(f"{'TrimImage ' + corners:44s} {ms:8.3f} ms" + ref_ms(src, 1), flush=True)
+    del x, src
