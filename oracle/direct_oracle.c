@@ -4,7 +4,7 @@
   The plain-C oracle of the two "directly applied" morphology methods of ImageMagick 7.1.1-45 Q16-HDRI, Distance (21) and
   Voronoi (22): MorphologyApply's special branch (morphology.c:3736-3776) around MorphologyPrimitiveDirect (:3242-3623),
   restated loop for loop.  It uses the main oracle's kernel struct, pixel_intensity and clamp_pixel, which are file-local
-  there, so this translation unit includes oracle.c.  Built by oracle/direct.mk into oracle/libdirect_oracle.so with the
+  there, so this translation unit includes oracle.c.  Built by oracle/Makefile into oracle/libdirect_oracle.so with the
   main oracle's flags (no contraction, standard excess precision); pinned bit for bit against the reference compiled from
   source by tests/test_oracle_direct_vs_ref.py.  Buffers as in oracle.h.
 

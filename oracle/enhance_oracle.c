@@ -6,7 +6,7 @@
   reference's operation order.  They are built on the colour restatements of the main oracle -- rgb_to_hsb / hsb_to_rgb
   and the other hue legs, rgb_to_xyz / xyz_to_lab / xyz_to_luv and their inverses, the illuminant table,
   decode_pixel_gamma / encode_pixel_gamma -- which are file-local there, so this translation unit includes oracle.c
-  itself rather than carrying a second copy of them.  Built by oracle/enhance.mk into oracle/libenhance_oracle.so with
+  itself rather than carrying a second copy of them.  Built by oracle/Makefile into oracle/libenhance_oracle.so with
   the main oracle's flags (no contraction, standard excess precision); pinned bit for bit against the reference compiled
   from source by tests/test_oracle_enhance_vs_ref.py.  Buffers as in oracle.h.
 

@@ -3,7 +3,7 @@
 
   The plain-C oracle of the last three image-returning accelerate hooks (accelerate-private.h:36-48): DespeckleImage,
   LocalContrastImage and WaveletDenoiseImage of ImageMagick 7.1.1-45 Q16-HDRI, restated in the reference's operation
-  order.  Built by oracle/hooks.mk into oracle/libhooks_oracle.so, next to the main oracle (oracle.c) and with the same
+  order.  Built by oracle/Makefile into oracle/libhooks_oracle.so, next to the main oracle (oracle.c) and with the same
   flags (no contraction, standard excess precision); pinned bit for bit against the reference compiled from source by
   tests/test_oracle_hooks_vs_ref.py.  Buffers as in oracle.h: tightly packed, channel-interleaved float32 Quantum,
   channels 1 Gray, 2 Gray+Alpha, 3 RGB, 4 RGBA.

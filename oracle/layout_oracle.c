@@ -5,7 +5,7 @@
   layout of the pixel cache -- GRAY, LinearGRAY and CMYK -- restated in the reference's operation order on top of the
   main oracle: its gamma curves (decode_pixel_gamma / encode_pixel_gamma), its PerceptibleReciprocal and, for every
   other space on either side of sRGB, orc_colorspace_ex itself.  Those are file-local there, so this translation unit
-  includes oracle.c rather than carrying a second copy of them.  Built by oracle/layout.mk into
+  includes oracle.c rather than carrying a second copy of them.  Built by oracle/Makefile into
   oracle/liblayout_oracle.so with the main oracle's flags (no contraction, standard excess precision); pinned bit for
   bit against the reference compiled from source by tests/test_oracle_layout_vs_ref.py.
 

@@ -5,7 +5,7 @@
   LevelizeImage, MinMaxStretchImage (AutoLevelImage), ContrastStretchImage (NormalizeImage), LinearStretchImage and
   GammaImage, restated in the reference's operation order.  It builds on the main oracle's pixel_intensity,
   perceptible_reciprocal, scale_quantum_to_map and scale_map_to_quantum, which are file-local there, so this translation
-  unit includes oracle.c.  Built by oracle/level.mk into oracle/liblevel_oracle.so with the main oracle's flags (no
+  unit includes oracle.c.  Built by oracle/Makefile into oracle/liblevel_oracle.so with the main oracle's flags (no
   contraction, standard excess precision); pinned bit for bit against the reference compiled from source by
   tests/test_oracle_level_vs_ref.py.  Buffers as in oracle.h; `update_mask` bit c = channel c has the Update trait;
   `per_channel` = the image's channel mask is not AllChannels.

@@ -3,8 +3,8 @@
 
   Driver of the UNMODIFIED reference's MorphologyImage with the directly applied methods, Distance (21) and Voronoi (22),
   on raw, tightly packed float buffers.  It uses the image helpers of oracle/ref_harness.c (make_image, export_image, the
-  BEGIN / END bracket), which are file-local there, so this translation unit includes it.  Built by oracle/direct.mk
-  against the reference archive that oracle/Makefile compiles from source, into oracle/_ref/libmagickref_direct.so.
+  BEGIN / END bracket), which are file-local there, so this translation unit includes it.  Built by oracle/Makefile
+  against the reference archive it compiles from source, into oracle/_ref/libmagickref_direct.so.
 */
 #include "ref_harness.c"
 

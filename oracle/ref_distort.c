@@ -3,7 +3,7 @@
 
   Driver of the UNMODIFIED reference's DistortImage and RotateImage on raw, tightly packed float buffers.  It uses the
   image helpers of oracle/ref_harness.c (make_image, the BEGIN / END bracket), which are file-local there, so this
-  translation unit includes it.  Built by oracle/distort.mk against the reference archive that oracle/Makefile compiles
+  translation unit includes it.  Built by oracle/Makefile against the reference archive it compiles
   from source, into oracle/_ref/libmagickref_distort.so.
 */
 #include "ref_harness.c"

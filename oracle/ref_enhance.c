@@ -3,8 +3,8 @@
 
   Drivers of the UNMODIFIED reference's ContrastImage, ModulateImage, GrayscaleImage and FunctionImage on raw, tightly
   packed float buffers, in place.  They use the image helpers of oracle/ref_harness.c (make_image, export_image, the
-  BEGIN / END bracket), which are file-local there, so this translation unit includes it.  Built by oracle/enhance.mk
-  against the reference archive that oracle/Makefile compiles from source, into oracle/_ref/libmagickref_enhance.so.
+  BEGIN / END bracket), which are file-local there, so this translation unit includes it.  Built by oracle/Makefile
+  against the reference archive it compiles from source, into oracle/_ref/libmagickref_enhance.so.
 */
 #include "ref_harness.c"
 

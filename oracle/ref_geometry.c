@@ -4,8 +4,8 @@
   Driver of the UNMODIFIED reference's orientation and crop operators (CropImage, ShaveImage, FlipImage, FlopImage,
   TransposeImage, TransverseImage, IntegralRotateImage, RollImage, AutoOrientImage) on raw, tightly packed float
   buffers.  It uses the image helpers of oracle/ref_harness.c (make_image, export_image, the BEGIN / END bracket), which
-  are file-local there, so this translation unit includes it.  Built by oracle/geometry.mk against the reference archive
-  that oracle/Makefile compiles from source, into oracle/_ref/libmagickref_geometry.so.
+  are file-local there, so this translation unit includes it.  Built by oracle/Makefile against the reference archive
+  it compiles from source, into oracle/_ref/libmagickref_geometry.so.
 */
 #include "ref_harness.c"
 

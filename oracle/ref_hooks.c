@@ -3,8 +3,8 @@
 
   Drivers of the UNMODIFIED reference's DespeckleImage, LocalContrastImage and WaveletDenoiseImage on raw, tightly
   packed float buffers (Quantum == float, channels interleaved; 1 Gray, 2 Gray+Alpha, 3 RGB, 4 RGBA), like
-  oracle/ref_harness.c does for the other operators.  Built by oracle/hooks.mk against the reference archive that
-  oracle/Makefile compiles from source, into oracle/_ref/libmagickref_hooks.so.
+  oracle/ref_harness.c does for the other operators.  Built by oracle/Makefile against the reference archive it
+  compiles from source, into oracle/_ref/libmagickref_hooks.so.
 */
 #include "MagickCore/studio.h"
 #include "MagickCore/MagickCore.h"

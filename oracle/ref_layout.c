@@ -5,7 +5,7 @@
   (GRAY, LinearGRAY, CMYK) on raw, tightly packed float buffers.  It reuses export_image and the BEGIN / END bracket of
   oracle/ref_harness.c, which are file-local there, so this translation unit includes it; images tagged GRAY,
   LinearGRAY or CMYK are built by its own helper, because their channel map is the colourspace's.  Built by
-  oracle/layout.mk against the reference archive that oracle/Makefile compiles from source, into
+  oracle/Makefile against the reference archive it compiles from source, into
   oracle/_ref/libmagickref_layout.so.
 */
 #include "ref_harness.c"

@@ -5,7 +5,7 @@
   ContrastStretchImage, NormalizeImage, LinearStretchImage and GammaImage on raw, tightly packed float buffers, in place,
   each under SetPixelChannelMask(channel_mask) (a ChannelType; -1 leaves the default mask).  They use the image helpers of
   oracle/ref_harness.c (make_image, export_image, the BEGIN / END bracket), which are file-local there, so this
-  translation unit includes it.  Built by oracle/level.mk against the reference archive that oracle/Makefile compiles
+  translation unit includes it.  Built by oracle/Makefile against the reference archive it compiles
   from source, into oracle/_ref/libmagickref_level.so.
 */
 #include "ref_harness.c"

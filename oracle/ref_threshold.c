@@ -4,8 +4,8 @@
   Drivers of the UNMODIFIED reference's AdaptiveThresholdImage, AutoThresholdImage, RangeThresholdImage and
   PerceptibleImage on raw, tightly packed float buffers, each under SetPixelChannelMask(channel_mask) (a ChannelType; -1
   leaves the default mask).  They use the image helpers of oracle/ref_harness.c (make_image, export_image, the BEGIN /
-  END bracket), which are file-local there, so this translation unit includes it.  Built by oracle/threshold.mk against
-  the reference archive that oracle/Makefile compiles from source, into oracle/_ref/libmagickref_threshold.so.
+  END bracket), which are file-local there, so this translation unit includes it.  Built by oracle/Makefile against
+  the reference archive it compiles from source, into oracle/_ref/libmagickref_threshold.so.
 */
 #include "ref_harness.c"
 

@@ -4,7 +4,7 @@
   Driver of the UNMODIFIED reference's GetImageBoundingBox (attribute.c:391) and TrimImage (transform.c:2412) on raw,
   tightly packed float buffers.  It uses the image helpers of oracle/ref_geometry.c (make_cmyk_image) and
   oracle/ref_harness.c (make_image, export_image, the BEGIN / END bracket), which are file-local there, so this
-  translation unit includes the former.  Built by oracle/trim.mk into oracle/_ref/libmagickref_trim.so.
+  translation unit includes the former.  Built by oracle/Makefile into oracle/_ref/libmagickref_trim.so.
 */
 #include "ref_geometry.c"
 

@@ -5,7 +5,7 @@
   7.1.1-45 Q16-HDRI): AdaptiveThresholdImage, AutoThresholdImage, RangeThresholdImage and PerceptibleImage, restated in
   the reference's operation order.  It builds on the main oracle's pixel_intensity, perceptible_reciprocal,
   scale_quantum_to_char and orc_threshold, which are file-local there, so this translation unit includes oracle.c.
-  Built by oracle/threshold.mk into oracle/libthreshold_oracle.so with the main oracle's flags (no contraction, standard
+  Built by oracle/Makefile into oracle/libthreshold_oracle.so with the main oracle's flags (no contraction, standard
   excess precision); pinned bit for bit against the reference compiled from source by
   tests/test_oracle_threshold_vs_ref.py.  Buffers as in oracle.h; `update_mask` bit c = channel c has the Update trait.
 

@@ -2,15 +2,11 @@
 (MorphologyPrimitiveDirect): the oracle-against-reference suite and the GPU suite run the same cases.
 
 The oracle is oracle/direct_oracle.c (oracle/libdirect_oracle.so) and the reference driver oracle/ref_direct.c
-(oracle/_ref/libmagickref_direct.so), both built by oracle/direct.mk.  What the reference computed for every case is stored
+(oracle/_ref/libmagickref_direct.so), both built by oracle/Makefile.  What the reference computed for every case is stored
 in tests/golden/direct_digests.json as "kernel/digest/channels/alpha_trait" (the digest of the head kernel the reference
 parsed, the digest of the resulting cache, its channel count and alpha trait), keyed like level_cases keys its own file;
 re-record it with MB200_RECORD_REFERENCE=1 where oracle/_ref is built."""
-import atexit
 import ctypes as C
-import json
-import os
-import subprocess
 
 import numpy as np
 
@@ -85,13 +81,7 @@ def sources(ch: int, w: int = 29, h: int = 23, seed: int = 3):
 def oracle():
     """The plain-C oracle; (re)built when stale."""
     if "oracle" not in _libs:
-        srcs = [ROOT / "oracle" / n for n in ("direct_oracle.c", "oracle.c", "oracle.h")]
-        if not ORACLE_SO.exists() or any(ORACLE_SO.stat().st_mtime < s.stat().st_mtime for s in srcs):
-            env = dict(os.environ)
-            env.pop("CC", None)
-            subprocess.run(["make", "-C", str(ROOT / "oracle"), "-f", "direct.mk", "port"], check=True, env=env,
-                           stdout=subprocess.DEVNULL)
-        o = C.CDLL(str(ORACLE_SO))
+        o = util.load_oracle(ORACLE_SO)
         o.orc_morphology_direct.argtypes = [_fp, _fp, _sz, _sz, _i, _i, C.POINTER(util.OrcKernel)]
         _libs["oracle"] = o
     return _libs["oracle"]
@@ -161,33 +151,5 @@ def ref_key(src, method, kernel: str) -> str:
     return result_key(digest(kernel_values(*util.ref_kernel(kernel))), *ref_run(src, method, kernel))
 
 
-_stored = None
-_recorded = {}
-
-
-def _save_recorded():
-    data = json.loads(DIGESTS.read_text()) if DIGESTS.exists() else {}
-    for (test, case), value in _recorded.items():
-        data.setdefault(test, {})[case] = value
-    DIGESTS.write_text("{\n" + ",\n".join(json.dumps(t) + ": " + json.dumps(c, separators=(",", ":"))
-                                           for t, c in sorted(data.items())) + "\n}\n")
-
-
-def reference(case: str, run, test: str = None):
-    """What the reference computed for `case` of the running test (or of `test`, "<file>::<test>[<params>]"), as
-    result_key().  With MB200_RECORD_REFERENCE=1 and the reference driver built, run() computes it with the reference
-    itself and the result is recorded when the process exits."""
-    global _stored
-    if test is None:
-        test = os.environ.get("PYTEST_CURRENT_TEST", "").rsplit(" (", 1)[0].split("::", 1)
-        test = test[0].rsplit("/", 1)[-1] + "::" + test[-1]
-    if os.environ.get("MB200_RECORD_REFERENCE") == "1" and REF_SO.exists():
-        if not _recorded:
-            atexit.register(_save_recorded)
-        _recorded[test, case] = run()
-        return _recorded[test, case]
-    if _stored is None:
-        _stored = json.loads(DIGESTS.read_text())
-    stored = _stored.get(test, {})
-    assert case in stored, f"no stored reference result for {test} / {case}"
-    return stored[case]
+# What the reference computed for `case` of the running test (or of `test`, "<file>::<test>[<params>]"), as result_key()
+reference = util.ReferenceStore(DIGESTS, REF_SO)

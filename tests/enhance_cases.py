@@ -2,14 +2,10 @@
 GrayscaleImage, FunctionImage): the oracle-against-reference suite and the GPU suite run the same cases.
 
 The oracle is oracle/enhance_oracle.c (oracle/libenhance_oracle.so) and the reference driver oracle/ref_enhance.c
-(oracle/_ref/libmagickref_enhance.so), both built by oracle/enhance.mk.  What the reference computed for every case is
+(oracle/_ref/libmagickref_enhance.so), both built by oracle/Makefile.  What the reference computed for every case is
 stored as a digest (util.digest) in tests/golden/enhance_digests.json, keyed like util.reference keys
 tests/golden/ref_digests.json; re-record it with MB200_RECORD_REFERENCE=1 where oracle/_ref is built."""
-import atexit
 import ctypes as C
-import json
-import os
-import subprocess
 
 import numpy as np
 
@@ -82,13 +78,7 @@ def mosaic(w: int, ch: int, seed: int = 11) -> np.ndarray:
 def oracle():
     """The plain-C oracle; (re)built when stale, like conftest.py does for oracle/liboracle.so."""
     if "oracle" not in _libs:
-        srcs = [ROOT / "oracle" / n for n in ("enhance_oracle.c", "oracle.c", "oracle.h")]
-        if not ORACLE_SO.exists() or any(ORACLE_SO.stat().st_mtime < s.stat().st_mtime for s in srcs):
-            env = dict(os.environ)
-            env.pop("CC", None)
-            subprocess.run(["make", "-C", str(ROOT / "oracle"), "-f", "enhance.mk", "port"], check=True, env=env,
-                           stdout=subprocess.DEVNULL)
-        o = C.CDLL(str(ORACLE_SO))
+        o = util.load_oracle(ORACLE_SO)
         o.orc_contrast.argtypes = [_fp, _sz, _sz, _i, _i]
         o.orc_modulate.argtypes = [_fp, _sz, _sz, _i, _d, _d, _d, _i, _i]
         o.orc_grayscale.argtypes = [_fp, _sz, _sz, _i, _i, _i]
@@ -109,35 +99,13 @@ def ref():
     return _libs["ref"]
 
 
-_stored = None
-_recorded = {}
-
-
-def _save_recorded():
-    data = json.loads(DIGESTS.read_text()) if DIGESTS.exists() else {}
-    for (test, case), value in _recorded.items():
-        data.setdefault(test, {})[case] = value
-    DIGESTS.write_text("{\n" + ",\n".join(json.dumps(t) + ": " + json.dumps(c, separators=(",", ":"))
-                                           for t, c in sorted(data.items())) + "\n}\n")
+_store = util.ReferenceStore(DIGESTS, REF_SO)
 
 
 def reference(case: str, run):
-    """Digest of what the reference computed for `case` of the running test (util.reference's scheme, own file).  With
-    MB200_RECORD_REFERENCE=1 and the reference driver built, run() computes it with the reference itself and the digest
-    is recorded when the process exits."""
-    global _stored
-    test = os.environ.get("PYTEST_CURRENT_TEST", "").rsplit(" (", 1)[0].split("::", 1)
-    test = test[0].rsplit("/", 1)[-1] + "::" + test[-1]
-    if os.environ.get("MB200_RECORD_REFERENCE") == "1" and REF_SO.exists():
-        if not _recorded:
-            atexit.register(_save_recorded)
-        _recorded[test, case] = digest(run())
-        return _recorded[test, case]
-    if _stored is None:
-        _stored = json.loads(DIGESTS.read_text())
-    stored = _stored.get(test, {})
-    assert case in stored, f"no stored reference result for {test} / {case}"
-    return stored[case]
+    """Digest of what the reference computed for `case` of the running test: of the output array run() returns with
+    the reference itself when recording."""
+    return _store(case, lambda: digest(run()))
 
 
 def modulate_percentages(geometry: str):

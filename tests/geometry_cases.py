@@ -2,14 +2,12 @@
 FlopImage, TransposeImage, TransverseImage, IntegralRotateImage, RollImage, AutoOrientImage): the planner-against-
 reference suite on the CPU and the GPU suite run the same cases.
 
-The reference driver is oracle/ref_geometry.c (oracle/_ref/libmagickref_geometry.so, built by oracle/geometry.mk).  What
+The reference driver is oracle/ref_geometry.c (oracle/_ref/libmagickref_geometry.so, built by oracle/Makefile).  What
 the reference computed for every case is stored in tests/golden/geometry_digests.json as "columns/rows/page_width/
 page_height/page_x/page_y/channels/digest", keyed by case name; the digest is over the raw 32-bit words, so NaN payloads
 and -0 count.  Re-record it with MB200_RECORD_REFERENCE=1 where oracle/_ref is built."""
 import ctypes as C
 import hashlib
-import json
-import os
 
 import numpy as np
 
@@ -111,30 +109,13 @@ def key(result) -> str:
     return "/".join(str(v) for v in g) + f"/{pixels.shape[2]}/{bits_digest(pixels)}"
 
 
-_stored = None
-_recorded = {}
-
-
-def _save_recorded():
-    data = json.loads(DIGESTS.read_text()) if DIGESTS.exists() else {}
-    data.update(_recorded)
-    DIGESTS.write_text("{\n" + ",\n".join(json.dumps(k) + ": " + json.dumps(v) for k, v in sorted(data.items())) + "\n}\n")
+_store = util.ReferenceStore(DIGESTS, REF_SO, by_test=False)
 
 
 def reference(case: str, run) -> str:
-    """What the reference computed for `case`, as key().  With MB200_RECORD_REFERENCE=1 and the reference driver built,
-    run() computes it with the reference itself and the result is recorded when the process exits."""
-    global _stored
-    if os.environ.get("MB200_RECORD_REFERENCE") == "1" and REF_SO.exists():
-        if not _recorded:
-            import atexit
-            atexit.register(_save_recorded)
-        _recorded[case] = key(run())
-        return _recorded[case]
-    if _stored is None:
-        _stored = json.loads(DIGESTS.read_text())
-    assert case in _stored, f"no stored reference result for {case}"
-    return _stored[case]
+    """What the reference computed for `case`, as key() of what run() returns with the reference itself when
+    recording."""
+    return _store(case, lambda: key(run()))
 
 
 def _case(out, name, layout, size, op, args=(), page=(0, 0, 0, 0)):

@@ -91,7 +91,8 @@ def main():
     out["kat/srgb"] = kat
     out["kat/lab"] = buf
     np.savez_compressed(OUT, **out)
-    print("wrote", OUT, OUT.stat().st_size, "bytes,", len(out), "arrays", len(util._recorded), "digests", r.ref_version())
+    print("wrote", OUT, OUT.stat().st_size, "bytes,", len(out), "arrays", len(util.REF_STORE.recorded), "digests",
+          r.ref_version())
 
 
 if __name__ == "__main__":

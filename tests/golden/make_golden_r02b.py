@@ -102,7 +102,7 @@ def main():
                 assert r.ref_colorspace(P(buf), W, H, ch, frm, to) == 0
                 util.record(f"r02b_golden/c{ch}", f"colorspace_{tag}", buf)
     np.savez_compressed(OUT, **out)
-    print(OUT, len(out), "arrays", OUT.stat().st_size, "bytes,", len(util._recorded), "digests")
+    print(OUT, len(out), "arrays", OUT.stat().st_size, "bytes,", len(util.REF_STORE.recorded), "digests")
 
 
 if __name__ == "__main__":

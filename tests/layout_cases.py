@@ -2,14 +2,10 @@
 layout (GRAY, LinearGRAY, CMYK): the oracle-against-reference suite and the GPU suite run the same cases.
 
 The oracle is oracle/layout_oracle.c (oracle/liblayout_oracle.so) and the reference driver oracle/ref_layout.c
-(oracle/_ref/libmagickref_layout.so), both built by oracle/layout.mk.  What the reference computed for every case is
+(oracle/_ref/libmagickref_layout.so), both built by oracle/Makefile.  What the reference computed for every case is
 stored as a digest (util.digest) in tests/golden/layout_digests.json, keyed like enhance_cases keys its own file;
 re-record it with MB200_RECORD_REFERENCE=1 where oracle/_ref is built."""
-import atexit
 import ctypes as C
-import json
-import os
-import subprocess
 
 import numpy as np
 
@@ -59,13 +55,7 @@ def source(colorspace: int, alpha: bool, w: int = 37, seed: int = 11) -> np.ndar
 def oracle():
     """The plain-C oracle; (re)built when stale."""
     if "oracle" not in _libs:
-        srcs = [ROOT / "oracle" / n for n in ("layout_oracle.c", "oracle.c", "oracle.h")]
-        if not ORACLE_SO.exists() or any(ORACLE_SO.stat().st_mtime < s.stat().st_mtime for s in srcs):
-            env = dict(os.environ)
-            env.pop("CC", None)
-            subprocess.run(["make", "-C", str(ROOT / "oracle"), "-f", "layout.mk", "port"], check=True, env=env,
-                           stdout=subprocess.DEVNULL)
-        o = C.CDLL(str(ORACLE_SO))
+        o = util.load_oracle(ORACLE_SO)
         o.orc_colorspace_channels.argtypes = [_i, _i]
         o.orc_colorspace_layout.argtypes = [_fp, _i, _fp, _i, _sz, _sz, _i, _i, C.c_void_p]
         _libs["oracle"] = o
@@ -107,36 +97,17 @@ def ref_layout(src, from_cs, to_cs, settings=None):
     return out.ravel()[: w * h * out_ch].reshape(h, w, out_ch).copy(), kind.value
 
 
-_stored = None
-_recorded = {}
+def result_key(pixels, kind) -> str:
+    return f"{digest(pixels)}/{kind}"
 
 
-def _save_recorded():
-    data = json.loads(DIGESTS.read_text()) if DIGESTS.exists() else {}
-    for (test, case), value in _recorded.items():
-        data.setdefault(test, {})[case] = value
-    DIGESTS.write_text("{\n" + ",\n".join(json.dumps(t) + ": " + json.dumps(c, separators=(",", ":"))
-                                           for t, c in sorted(data.items())) + "\n}\n")
+_store = util.ReferenceStore(DIGESTS, REF_SO)
 
 
 def reference(case: str, run):
     """What the reference computed for `case` of the running test: the digest of its pixels and the image type, as
-    "digest/type".  With MB200_RECORD_REFERENCE=1 and the reference driver built, run() computes it with the reference
-    itself and the result is recorded when the process exits."""
-    global _stored
-    test = os.environ.get("PYTEST_CURRENT_TEST", "").rsplit(" (", 1)[0].split("::", 1)
-    test = test[0].rsplit("/", 1)[-1] + "::" + test[-1]
-    if os.environ.get("MB200_RECORD_REFERENCE") == "1" and REF_SO.exists():
-        if not _recorded:
-            atexit.register(_save_recorded)
-        pixels, kind = run()
-        _recorded[test, case] = f"{digest(pixels)}/{kind}"
-        return _recorded[test, case]
-    if _stored is None:
-        _stored = json.loads(DIGESTS.read_text())
-    stored = _stored.get(test, {})
-    assert case in stored, f"no stored reference result for {test} / {case}"
-    return stored[case]
+    result_key() of the (pixels, type) run() returns with the reference itself when recording."""
+    return _store(case, lambda: result_key(*run()))
 
 
 # ImageType (MagickCore/image.h:38-51) the reference leaves for a layout target: GrayscaleType for GRAY / LinearGRAY,

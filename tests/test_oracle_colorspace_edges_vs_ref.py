@@ -12,10 +12,7 @@ The reference's results are stored in tests/golden/colorspace_edge_digests.json;
     MB200_RECORD_REFERENCE=1 python -m pytest tests/test_oracle_colorspace_edges_vs_ref.py
 
 where oracle/_ref is built."""
-import atexit
 import ctypes as C
-import json
-import os
 
 import numpy as np
 import pytest
@@ -25,40 +22,12 @@ import util
 from util import P, ROOT, digest
 
 DIGESTS = ROOT / "tests" / "golden" / "colorspace_edge_digests.json"
-_stored = None
-_recorded = {}
+# "<digest>/<zero-sign digest>" of what the reference computed for each case of the running test
+reference = util.ReferenceStore(DIGESTS, util.REF_SO)
 
 
-def _save_recorded():
-    data = json.loads(DIGESTS.read_text()) if DIGESTS.exists() else {}
-    for (test, case), value in _recorded.items():
-        data.setdefault(test, {})[case] = value
-    DIGESTS.write_text("{\n" + ",\n".join(json.dumps(t) + ": " + json.dumps(c, separators=(",", ":"))
-                                           for t, c in sorted(data.items())) + "\n}\n")
-
-
-def _signs(a):
-    return digest((a == 0) & np.signbit(a))
-
-
-def reference(case, run):
-    """"<digest>/<zero-sign digest>" of what the reference computed for `case` of the running test.  With
-    MB200_RECORD_REFERENCE=1 and oracle/_ref built, run() computes it with the reference and it is recorded when the
-    process exits."""
-    global _stored
-    test = os.environ.get("PYTEST_CURRENT_TEST", "").rsplit(" (", 1)[0].split("::", 1)
-    test = test[0].rsplit("/", 1)[-1] + "::" + test[-1]
-    if os.environ.get("MB200_RECORD_REFERENCE") == "1" and util.have_ref():
-        if not _recorded:
-            atexit.register(_save_recorded)
-        out = run()
-        _recorded[test, case] = f"{digest(out)}/{_signs(out)}"
-        return _recorded[test, case]
-    if _stored is None:
-        _stored = json.loads(DIGESTS.read_text())
-    stored = _stored.get(test, {})
-    assert case in stored, f"no stored reference result for {test} / {case}"
-    return stored[case]
+def key(a):
+    return f"{digest(a)}/{util.zero_signs(a)}"
 
 
 def orc(src, frm, to, values=None):
@@ -84,7 +53,7 @@ def check(src, frm, to, case, settings=None):
     got = orc(src, frm, to, values)
     if src.shape[2] == 4:
         assert np.array_equal(got[..., 3].view(np.int32), src[..., 3].view(np.int32)), case     # alpha untouched
-    assert f"{digest(got)}/{_signs(got)}" == reference(case, lambda: ref(src, frm, to, defines)), case
+    assert key(got) == reference(case, lambda: key(ref(src, frm, to, defines))), case
     return got
 
 

@@ -2,20 +2,17 @@
 (effect.c:2013) and WaveletDenoiseImage (visual-effects.c:3515) -- against the reference, bit for bit.
 
 The oracle is oracle/hooks_oracle.c (oracle/libhooks_oracle.so) and the reference driver oracle/ref_hooks.c
-(oracle/_ref/libmagickref_hooks.so), both built by oracle/hooks.mk.  What the reference computed for every case is stored
+(oracle/_ref/libmagickref_hooks.so), both built by oracle/Makefile.  What the reference computed for every case is stored
 as a digest (util.digest) in tests/golden/hook_digests.json, keyed like util.reference keys tests/golden/ref_digests.json;
 re-record it with MB200_RECORD_REFERENCE=1 where oracle/_ref is built."""
 from __future__ import annotations
 
-import atexit
 import ctypes as C
-import json
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
+import util
 from util import P, ROOT, digest, make_image
 
 _fp, _sz, _d, _i = C.POINTER(C.c_float), C.c_size_t, C.c_double, C.c_int
@@ -28,13 +25,7 @@ _libs = {}
 def oracle():
     """The plain-C oracle; (re)built when stale, like conftest.py does for oracle/liboracle.so."""
     if "oracle" not in _libs:
-        src = ROOT / "oracle" / "hooks_oracle.c"
-        if not ORACLE_SO.exists() or ORACLE_SO.stat().st_mtime < src.stat().st_mtime:
-            env = dict(os.environ)
-            env.pop("CC", None)
-            subprocess.run(["make", "-C", str(ROOT / "oracle"), "-f", "hooks.mk", "port"], check=True, env=env,
-                           stdout=subprocess.DEVNULL)
-        o = C.CDLL(str(ORACLE_SO))
+        o = util.load_oracle(ORACLE_SO)
         o.orc_despeckle.argtypes = [_fp, _fp, _sz, _sz, _i]
         o.orc_local_contrast.argtypes = [_fp, _fp, _sz, _sz, _i, _d, _d]
         o.orc_wavelet_denoise.argtypes = [_fp, _fp, _sz, _sz, _i, _d, _d]
@@ -53,35 +44,13 @@ def ref():
     return _libs["ref"]
 
 
-_stored = None
-_recorded = {}
-
-
-def _save_recorded():
-    data = json.loads(DIGESTS.read_text()) if DIGESTS.exists() else {}
-    for (test, case), value in _recorded.items():
-        data.setdefault(test, {})[case] = value
-    DIGESTS.write_text("{\n" + ",\n".join(json.dumps(t) + ": " + json.dumps(c, separators=(",", ":"))
-                                           for t, c in sorted(data.items())) + "\n}\n")
+_store = util.ReferenceStore(DIGESTS, REF_SO)
 
 
 def reference(case: str, run):
-    """Digest of what the reference computed for `case` of the running test (util.reference's scheme, own file).  With
-    MB200_RECORD_REFERENCE=1 and the reference driver built, run() computes it with the reference itself and the digest
-    is recorded when the process exits."""
-    global _stored
-    test = os.environ.get("PYTEST_CURRENT_TEST", "").rsplit(" (", 1)[0].split("::", 1)
-    test = test[0].rsplit("/", 1)[-1] + "::" + test[-1]
-    if os.environ.get("MB200_RECORD_REFERENCE") == "1" and REF_SO.exists():
-        if not _recorded:
-            atexit.register(_save_recorded)
-        _recorded[test, case] = digest(run())
-        return _recorded[test, case]
-    if _stored is None:
-        _stored = json.loads(DIGESTS.read_text())
-    stored = _stored.get(test, {})
-    assert case in stored, f"no stored reference result for {test} / {case}"
-    return stored[case]
+    """Digest of what the reference computed for `case` of the running test: of the output array run() returns with
+    the reference itself when recording."""
+    return _store(case, lambda: digest(run()))
 
 
 def hook_image(w, h, ch, kind, seed=5):

@@ -4,8 +4,8 @@ whole NaN rows and columns, infinite alpha lines, blocks whose products are all 
 sources, reductions to one row or column, same-size resizes with a filter, the regular table's threshold, factors one
 double ULP apart, and every filter.  The GPU suite (test_gpu_resample_edges.py) compares the kernels with this oracle.
 
-Each result is stored as "<digest>/<zero-sign digest>" (test_oracle_stencil_edges_vs_ref.reference) in
-tests/golden/resample_edge_digests.json, since util.digest hashes -0 as +0; re-record them with
+Each result is stored as "<digest>/<zero-sign digest>" (util.zero_signs) in tests/golden/resample_edge_digests.json,
+since util.digest hashes -0 as +0; re-record them with
 
     MB200_RECORD_REFERENCE=1 python -m pytest tests/test_oracle_resample_edges_vs_ref.py
 
@@ -14,11 +14,14 @@ import numpy as np
 import pytest
 
 import resample_edge_cases as rc
-import test_oracle_stencil_edges_vs_ref as stencil
 import util
 from util import P, digest
 
-DIGESTS = util.ROOT / "tests" / "golden" / "resample_edge_digests.json"
+reference = util.ReferenceStore(util.ROOT / "tests" / "golden" / "resample_edge_digests.json", util.REF_SO)
+
+
+def key(a):
+    return f"{digest(a)}/{util.zero_signs(a)}"
 
 
 def _run(lib, name, src, ow, oh, *args):
@@ -30,8 +33,8 @@ def _run(lib, name, src, ow, oh, *args):
 
 def check(op, src, ow, oh, args, case):
     got = _run(util.oracle(), "orc_" + op, src, ow, oh, *args)
-    want = stencil.reference(case, lambda: _run(util.ref(), "ref_" + op, src, ow, oh, *args), DIGESTS)
-    assert f"{digest(got)}/{stencil._signs(got)}" == want, case
+    want = reference(case, lambda: key(_run(util.ref(), "ref_" + op, src, ow, oh, *args)))
+    assert key(got) == want, case
 
 
 @pytest.mark.parametrize("ch", [1, 2, 3, 4])

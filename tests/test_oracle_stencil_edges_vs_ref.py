@@ -14,10 +14,6 @@ The reference's results are stored in tests/golden/stencil_edge_digests.json; re
     MB200_RECORD_REFERENCE=1 python -m pytest tests/test_oracle_stencil_edges_vs_ref.py
 
 where oracle/_ref is built."""
-import atexit
-import json
-import os
-
 import numpy as np
 import pytest
 
@@ -26,41 +22,12 @@ import util
 from util import P, ROOT, digest
 
 DIGESTS = ROOT / "tests" / "golden" / "stencil_edge_digests.json"
-_stored = {}                    # digest file -> its contents
-_recorded = {}                  # digest file -> {(test, case): result}
+# "<digest>/<zero-sign digest>" of what the reference computed for each case of the running test
+reference = util.ReferenceStore(DIGESTS, util.REF_SO)
 
 
-def _save_recorded():
-    for path, recorded in _recorded.items():
-        data = json.loads(path.read_text()) if path.exists() else {}
-        for (test, case), value in recorded.items():
-            data.setdefault(test, {})[case] = value
-        path.write_text("{\n" + ",\n".join(json.dumps(t) + ": " + json.dumps(c, separators=(",", ":"))
-                                            for t, c in sorted(data.items())) + "\n}\n")
-
-
-def _signs(a):
-    return digest((a == 0) & np.signbit(a))
-
-
-def reference(case, run, digests=DIGESTS):
-    """"<digest>/<zero-sign digest>" of what the reference computed for `case` of the running test, stored in the file
-    `digests`.  With MB200_RECORD_REFERENCE=1 and oracle/_ref built, run() computes it with the reference and it is
-    recorded when the process exits."""
-    test = os.environ.get("PYTEST_CURRENT_TEST", "").rsplit(" (", 1)[0].split("::", 1)
-    test = test[0].rsplit("/", 1)[-1] + "::" + test[-1]
-    if os.environ.get("MB200_RECORD_REFERENCE") == "1" and util.have_ref():
-        if not _recorded:
-            atexit.register(_save_recorded)
-        out = run()
-        recorded = _recorded.setdefault(digests, {})
-        recorded[test, case] = f"{digest(out)}/{_signs(out)}"
-        return recorded[test, case]
-    if digests not in _stored:
-        _stored[digests] = json.loads(digests.read_text())
-    stored = _stored[digests].get(test, {})
-    assert case in stored, f"no stored reference result for {test} / {case}"
-    return stored[case]
+def key(a):
+    return f"{digest(a)}/{util.zero_signs(a)}"
 
 
 def _call(lib, name, src, args):
@@ -79,8 +46,8 @@ def _masked(out, src, op, args):
 
 def check(op, src, args, case):
     got = _masked(_call(util.oracle(), "orc_" + op, src, args), src, op, args)
-    want = reference(case, lambda: _masked(_call(util.ref(), "ref_" + op, src, args), src, op, args))
-    assert f"{digest(got)}/{_signs(got)}" == want, case
+    want = reference(case, lambda: key(_masked(_call(util.ref(), "ref_" + op, src, args), src, op, args)))
+    assert key(got) == want, case
 
 
 @pytest.mark.parametrize("ch", [1, 2, 3, 4])

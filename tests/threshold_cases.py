@@ -2,14 +2,10 @@
 RangeThresholdImage and PerceptibleImage: the oracle-against-reference suite and the GPU suite run the same cases.
 
 The oracle is oracle/threshold_oracle.c (oracle/libthreshold_oracle.so) and the reference driver oracle/ref_threshold.c
-(oracle/_ref/libmagickref_threshold.so), both built by oracle/threshold.mk.  What the reference computed for every case
+(oracle/_ref/libmagickref_threshold.so), both built by oracle/Makefile.  What the reference computed for every case
 is stored in tests/golden/threshold_digests.json as "digest/channels/property"; re-record it with
 MB200_RECORD_REFERENCE=1 where oracle/_ref is built."""
-import atexit
 import ctypes as C
-import json
-import os
-import subprocess
 
 import numpy as np
 
@@ -133,13 +129,7 @@ def update_mask(channel_mask: int, ch: int) -> int:
 def oracle():
     """The plain-C oracle; (re)built when stale."""
     if "oracle" not in _libs:
-        srcs = [ROOT / "oracle" / n for n in ("threshold_oracle.c", "oracle.c", "oracle.h")]
-        if not ORACLE_SO.exists() or any(ORACLE_SO.stat().st_mtime < s.stat().st_mtime for s in srcs):
-            env = dict(os.environ)
-            env.pop("CC", None)
-            subprocess.run(["make", "-C", str(ROOT / "oracle"), "-f", "threshold.mk", "port"], check=True, env=env,
-                           stdout=subprocess.DEVNULL)
-        o = C.CDLL(str(ORACLE_SO))
+        o = util.load_oracle(ORACLE_SO)
         o.orc_adaptive_threshold.argtypes = [_fp, _fp, _sz, _sz, _i, _sz, _sz, _d, _u]
         o.orc_auto_threshold.argtypes = [_fp, _sz, _sz, _i, _i, _dp]
         o.orc_range_threshold.argtypes = [_fp, _sz, _sz, _i, _d, _d, _d, _d, _i, _u]
@@ -193,32 +183,10 @@ def result_key(pixels, prop) -> str:
     return f"{digest(pixels)}/{pixels.shape[2]}/{prop}"
 
 
-_stored = None
-_recorded = {}
-
-
-def _save_recorded():
-    data = json.loads(DIGESTS.read_text()) if DIGESTS.exists() else {}
-    for (test, case), value in _recorded.items():
-        data.setdefault(test, {})[case] = value
-    DIGESTS.write_text("{\n" + ",\n".join(json.dumps(t) + ": " + json.dumps(c, separators=(",", ":"))
-                                           for t, c in sorted(data.items())) + "\n}\n")
+_store = util.ReferenceStore(DIGESTS, REF_SO)
 
 
 def reference(case: str, run):
-    """What the reference computed for `case` of the running test, as result_key() of its (pixels, property).  With
-    MB200_RECORD_REFERENCE=1 and the reference driver built, run() computes it with the reference itself and the result
-    is recorded when the process exits."""
-    global _stored
-    test = os.environ.get("PYTEST_CURRENT_TEST", "").rsplit(" (", 1)[0].split("::", 1)
-    test = test[0].rsplit("/", 1)[-1] + "::" + test[-1]
-    if os.environ.get("MB200_RECORD_REFERENCE") == "1" and REF_SO.exists():
-        if not _recorded:
-            atexit.register(_save_recorded)
-        _recorded[test, case] = result_key(*run())
-        return _recorded[test, case]
-    if _stored is None:
-        _stored = json.loads(DIGESTS.read_text())
-    stored = _stored.get(test, {})
-    assert case in stored, f"no stored reference result for {test} / {case}"
-    return stored[case]
+    """What the reference computed for `case` of the running test, as result_key() of the (pixels, property) run()
+    returns with the reference itself when recording."""
+    return _store(case, lambda: result_key(*run()))

@@ -1,14 +1,12 @@
 """Cases and runners shared by the tests of GetImageBoundingBox and TrimImage: the host suite (NumPy row summaries,
 mb200_bounding_box_from_rows and mb200_trim_plan) and the GPU suite run the same cases.
 
-The reference driver is oracle/ref_trim.c (oracle/_ref/libmagickref_trim.so, built by oracle/trim.mk), run with one
+The reference driver is oracle/ref_trim.c (oracle/_ref/libmagickref_trim.so, built by oracle/Makefile), run with one
 thread (the reference's threaded result depends on the OpenMP schedule; see there).  What the reference computed for
 every case is stored in tests/golden/trim_digests.json, keyed by case name: the bounding box and the exception severity afterwards as "width/height/x/y/severity"; for a case that also trims,
 under "trim <name>", TrimImage's result in the geometry_cases.key format followed by "/severity".  Re-record it with
 MB200_RECORD_REFERENCE=1 where oracle/_ref is built."""
 import ctypes as C
-import json
-import os
 
 import numpy as np
 
@@ -130,30 +128,8 @@ def ref_trim_key(case) -> str:
     return gc.key((out[: cols * rows * n].reshape(rows, cols, n), geom)) + f"/{sev}"
 
 
-_stored = None
-_recorded = {}
-
-
-def _save_recorded():
-    data = json.loads(DIGESTS.read_text()) if DIGESTS.exists() else {}
-    data.update(_recorded)
-    DIGESTS.write_text("{\n" + ",\n".join(json.dumps(k) + ": " + json.dumps(v) for k, v in sorted(data.items())) + "\n}\n")
-
-
-def reference(name: str, run) -> str:
-    """What the reference computed for `name`.  With MB200_RECORD_REFERENCE=1 and the reference driver built, run()
-    computes it with the reference itself and the result is recorded when the process exits."""
-    global _stored
-    if os.environ.get("MB200_RECORD_REFERENCE") == "1" and REF_SO.exists():
-        if not _recorded:
-            import atexit
-            atexit.register(_save_recorded)
-        _recorded[name] = run()
-        return _recorded[name]
-    if _stored is None:
-        _stored = json.loads(DIGESTS.read_text())
-    assert name in _stored, f"no stored reference result for {name}"
-    return _stored[name]
+# What the reference computed for a case name, as ref_box_key() or, under "trim <name>", ref_trim_key()
+reference = util.ReferenceStore(DIGESTS, REF_SO, by_test=False)
 
 
 def box_reference(name, case) -> str:

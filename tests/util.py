@@ -6,6 +6,7 @@ import ctypes as C
 import hashlib
 import json
 import os
+import subprocess
 from pathlib import Path
 
 import numpy as np
@@ -94,6 +95,22 @@ def oracle() -> C.CDLL:
     return _oracle
 
 
+_port_built = False
+
+
+def load_oracle(path: Path) -> C.CDLL:
+    """The plain-C oracle library `path` (oracle/lib*.so), once `make port` has brought every oracle library up to date
+    (run once per process: make decides what is stale)."""
+    global _port_built
+    if not _port_built:
+        env = dict(os.environ)
+        env.pop("CC", None)
+        subprocess.run(["make", "-s", "-C", str(ROOT / "oracle"), "port"], check=True, env=env,
+                       stdout=subprocess.DEVNULL)
+        _port_built = True
+    return C.CDLL(str(path))
+
+
 def have_ref() -> bool:
     return REF_SO.exists()
 
@@ -147,46 +164,81 @@ def digest(a: np.ndarray) -> str:
     return h.hexdigest()[:10]
 
 
-_ref_digests = None
-_recorded = {}
+def current_test() -> str:
+    """The running test as "<file>::<test>[<parameter id>]": its node id without the directory and the phase."""
+    test = os.environ.get("PYTEST_CURRENT_TEST", "").rsplit(" (", 1)[0].split("::", 1)
+    return test[0].rsplit("/", 1)[-1] + "::" + test[-1]
 
 
-def _save_recorded():
-    data = json.loads(REF_DIGESTS.read_text()) if REF_DIGESTS.exists() else {}
-    for (test, case), value in _recorded.items():
-        data.setdefault(test, {})[case] = value
-    REF_DIGESTS.write_text("{\n" + ",\n".join(json.dumps(t) + ": " + json.dumps(c, separators=(",", ":"))
-                                               for t, c in sorted(data.items())) + "\n}\n")
+def zero_signs(a: np.ndarray) -> str:
+    """Digest of where the zeros of `a` are negative: digest() hashes -0 as +0, so this pins the sign of a zero."""
+    return digest((a == 0) & np.signbit(a))
+
+
+class ReferenceStore:
+    """What the reference computed, stored as strings in the JSON file `path`: nested as {"<file>::<test>[<params>]":
+    {case: value}} (by_test, the running test's or `test`'s entries) or flat as {case: value}.
+
+    store(case, run, test=None) returns the stored value and asserts there is one.  With MB200_RECORD_REFERENCE=1 and
+    the reference library `ref_so` built, it returns run() instead, which computes the value with the reference itself,
+    and records it into `path` (merged into what is there) when the process exits."""
+
+    def __init__(self, path: Path, ref_so: Path, by_test: bool = True):
+        self.path, self.ref_so, self.by_test = path, ref_so, by_test
+        self.stored = None
+        self.recorded = {}
+
+    def entries(self, test: str = None) -> dict:
+        """case -> value of `test` (nested), or of the whole file (flat)."""
+        if self.stored is None:
+            self.stored = json.loads(self.path.read_text())
+        return self.stored.get(test, {}) if self.by_test else self.stored
+
+    def __call__(self, case: str, run, test: str = None) -> str:
+        if self.by_test and test is None:
+            test = current_test()
+        if os.environ.get("MB200_RECORD_REFERENCE") == "1" and self.ref_so.exists():
+            return self.record(case, run(), test)
+        stored = self.entries(test)
+        assert case in stored, "no stored reference result for " + (f"{test} / {case}" if self.by_test else case)
+        return stored[case]
+
+    def record(self, case: str, value: str, test: str = None) -> str:
+        if not self.recorded:
+            atexit.register(self._save)
+        self.recorded[(test, case) if self.by_test else case] = value
+        return value
+
+    def _save(self):
+        data = json.loads(self.path.read_text()) if self.path.exists() else {}
+        if self.by_test:
+            for (test, case), value in self.recorded.items():
+                data.setdefault(test, {})[case] = value
+            lines = (json.dumps(t) + ": " + json.dumps(c, separators=(",", ":")) for t, c in sorted(data.items()))
+        else:
+            data.update(self.recorded)
+            lines = (json.dumps(k) + ": " + json.dumps(v) for k, v in sorted(data.items()))
+        self.path.write_text("{\n" + ",\n".join(lines) + "\n}\n")
+
+
+REF_STORE = ReferenceStore(REF_DIGESTS, REF_SO)
 
 
 def record(group: str, case: str, a: np.ndarray) -> str:
     """Stores the digest of the reference's output `a` as `group` / `case` of tests/golden/ref_digests.json (written
     when the process exits)."""
-    if not _recorded:
-        atexit.register(_save_recorded)
-    _recorded[group, case] = digest(a)
-    return _recorded[group, case]
+    return REF_STORE.record(case, digest(a), group)
 
 
 def stored_digests(group: str) -> dict:
-    global _ref_digests
-    if _ref_digests is None:
-        _ref_digests = json.loads(REF_DIGESTS.read_text())
-    return _ref_digests.get(group, {})
+    return REF_STORE.entries(group)
 
 
 def reference(case: str, run):
     """Digest of what the reference computed for `case` of the running test, from tests/golden/ref_digests.json.
     With MB200_RECORD_REFERENCE=1 and oracle/_ref built, run() computes it with the reference itself (it returns the
     output array) and the digest is recorded into that file when the process exits."""
-    # "<path>::<test>[<parameter id>] (<phase>)": the node id without its directory and without the phase
-    test = os.environ.get("PYTEST_CURRENT_TEST", "").rsplit(" (", 1)[0].split("::", 1)
-    test = test[0].rsplit("/", 1)[-1] + "::" + test[-1]
-    if os.environ.get("MB200_RECORD_REFERENCE") == "1" and have_ref():
-        return record(test, case, run())
-    stored = stored_digests(test)
-    assert case in stored, f"no stored reference result for {test} / {case}"
-    return stored[case]
+    return REF_STORE(case, lambda: digest(run()))
 
 
 def ref_kernel(string: str, idx: int = 0):
