@@ -26,7 +26,7 @@ NVCC_FLAGS = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC,-fvisibilit
               "-Xptxas", "-v"]
 
 SOURCES = ["runtime.cu", "kernel_info.cpp", "resize_filter.cpp", "resize_tables.cpp", "conv1d.cu", "conv_mma.cu",
-           "morph2d.cu", "morph_stream.cu", "morph_direct.cu", "cache.cu", "resize.cu", "resize_stream.cu", "colorspace.cu", "hexcone.cu", "pointwise.cu", "equalize.cu", "stencils.cu", "hooks.cu", "enhance.cu", "layout.cu", "level.cu",
+           "morph2d.cu", "morph_stream.cu", "morph_direct.cu", "cache.cu", "resize.cu", "resize_stream.cu", "colorspace.cu", "hexcone.cu", "pointwise.cu", "stencils.cu", "hooks.cu", "enhance.cu", "layout.cu", "level.cu",
            "distort_plan.cpp", "distort.cu", "geometry_plan.cpp", "geometry.cu", "threshold.cu", "trim.cu", "api.cu"]
 # distort.cu restates the reference's EWA sampler operation by operation: no contraction into fused multiply-adds.
 FILE_FLAGS = {"distort.cu": ["-fmad=false"], "threshold.cu": ["-fmad=false"], "trim.cu": ["-fmad=false"]}

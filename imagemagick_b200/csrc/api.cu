@@ -10,7 +10,7 @@
 //   TransformImageColorspace MagickCore/colorspace.c:1751
 // Intermediates live in HBM as float Quantum, exactly like the reference's intermediate
 // images (the rounding between passes is part of the semantics).
-#include "mb200_internal.h"
+#include "launch.cuh"
 
 #include <cuda_runtime.h>
 
@@ -22,20 +22,6 @@
 using namespace mb200;
 
 namespace {
-
-struct StreamAlloc {           // stream-ordered temporary; freed (stream-ordered) on scope exit
-  void *ptr = nullptr;
-  cudaStream_t s;
-  explicit StreamAlloc(cudaStream_t stream) : s(stream) {}
-  int alloc(size_t bytes) {
-    cudaError_t e = cudaMallocAsync(&ptr, bytes ? bytes : 1, temp_pool(), s);      // the library's private pool
-    if (e != cudaSuccess) { ptr = nullptr; return cuda_fail(e, "cudaMallocAsync"); }
-    return MB200_OK;
-  }
-  ~StreamAlloc() { if (ptr) cudaFreeAsync(ptr, s); }
-  StreamAlloc(const StreamAlloc &) = delete;
-  StreamAlloc &operator=(const StreamAlloc &) = delete;
-};
 
 int prepare(void *stream, cudaStream_t *out) {
   int rc = ensure_device();
@@ -1057,11 +1043,9 @@ int mb200_resize_copy_channels_dev(const float *src, size_t width, size_t height
   for (size_t i = 0; i < out_width; ++i) table[i] = static_cast<int>(nx[i]);
   for (size_t i = 0; i < out_height; ++i) table[out_width + i] = static_cast<int>(ny[i]);
   StreamAlloc d_table(s);
-  rc = d_table.alloc(table.size() * sizeof(int));
+  rc = d_table.upload(table.data(), table.size() * sizeof(int), "resize copy channels: table upload");
   if (rc) return rc;
-  cudaError_t e = cudaMemcpyAsync(d_table.ptr, table.data(), table.size() * sizeof(int), cudaMemcpyHostToDevice, s);
-  if (e != cudaSuccess) return cuda_fail(e, "resize copy channels: table upload");
-  const int *d = static_cast<const int *>(d_table.ptr);
+  const int *d = d_table.as<int>();
   return launch_resize_copy_channels(dst, src, width, out_width, out_height, channels, d, d + out_width, update_mask, s);
 }
 
@@ -1297,14 +1281,11 @@ int mb200_scale_image_dev(const float *src, size_t width, size_t height, int cha
   for (size_t i = 0; i <= out_width; ++i) xo[i] = static_cast<int>(xoff[i]);
   for (size_t i = 0; i <= out_height; ++i) yo[i] = static_cast<int>(yoff[i]);
   StreamAlloc d_ints(s), d_wts(s);
-  rc = d_ints.alloc(ints.size() * sizeof(int));
-  if (!rc) rc = d_wts.alloc(wts.size() * sizeof(double));
+  rc = d_ints.upload(ints.data(), ints.size() * sizeof(int), "scale: table upload");
+  if (!rc) rc = d_wts.upload(wts.data(), wts.size() * sizeof(double), "scale: table upload");
   if (rc) return rc;
-  cudaError_t e = cudaMemcpyAsync(d_ints.ptr, ints.data(), ints.size() * sizeof(int), cudaMemcpyHostToDevice, s);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(d_wts.ptr, wts.data(), wts.size() * sizeof(double), cudaMemcpyHostToDevice, s);
-  if (e != cudaSuccess) return cuda_fail(e, "scale: table upload");
-  const int *di = static_cast<const int *>(d_ints.ptr);
-  const double *dw = static_cast<const double *>(d_wts.ptr);
+  const int *di = d_ints.as<int>();
+  const double *dw = d_wts.as<double>();
   return launch_scale(src, width, height, channels, dst, out_width, out_height, di, di + out_width + 1 + out_height + 1, dw,
                       di + out_width + 1, di + out_width + 1 + out_height + 1 + nx, dw + nx, s);
 }

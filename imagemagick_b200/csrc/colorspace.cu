@@ -14,7 +14,7 @@
 // 100, 255 ...) become multiplications by the rounded reciprocal, and the reference's only libm
 // call, pow(t,1/3), is a fp32 MUFU seed refined by one Newton step on t^(-1/3) in FP64.
 // Alpha is untouched.  One thread per pixel, float4 access for RGBA; FP64-pipe bound.
-#include "mb200_internal.h"
+#include "launch.cuh"
 #include "colorspace_math.cuh"
 
 #include <cuda_runtime.h>
@@ -217,10 +217,7 @@ int launch_mode(float *buf, size_t npixels, int channels, cudaStream_t s) {
   const unsigned blocks = static_cast<unsigned>((npixels + 256 * kPixels - 1) / (256 * kPixels));
   if (channels == 4) colorspace_kernel<4, MODE><<<blocks, 256, 0, s>>>(buf, npixels);
   else colorspace_kernel<3, MODE><<<blocks, 256, 0, s>>>(buf, npixels);
-  count_launch();
-  const cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return cuda_fail(e, "colorspace launch");
-  return MB200_OK;
+  return launch_status("colorspace launch");
 }
 
 // ---- XYZ-derived spaces of the generic branch: Adobe98, DisplayP3, ProPhoto (an RGB matrix and the sRGB transfer curve on
@@ -435,10 +432,7 @@ int launch_xyz_family_leg(float *buf, size_t npixels, int channels, int space, b
   const unsigned blocks = static_cast<unsigned>((npixels + 255) / 256);
   if (channels == 4) xyz_family_kernel<4><<<blocks, 256, 0, s>>>(buf, npixels, space, forward ? 1 : 0, st);
   else xyz_family_kernel<3><<<blocks, 256, 0, s>>>(buf, npixels, space, forward ? 1 : 0, st);
-  count_launch();
-  const cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return cuda_fail(e, "colorspace launch");
-  return MB200_OK;
+  return launch_status("colorspace launch");
 }
 
 // ---- matrix colourspaces: CMY, YCbCr (= YPbPr), YDbDr, YIQ, YPbPr, YUV through the generic branch
@@ -566,10 +560,7 @@ int launch_matrix_leg(float *buf, size_t npixels, int channels, const MatrixLeg 
   const unsigned blocks = static_cast<unsigned>((npixels + 255) / 256);
   if (channels == 4) matrix_leg_kernel<4><<<blocks, 256, 0, s>>>(buf, npixels, leg);
   else matrix_leg_kernel<3><<<blocks, 256, 0, s>>>(buf, npixels, leg);
-  count_launch();
-  const cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return cuda_fail(e, "colorspace launch");
-  return MB200_OK;
+  return launch_status("colorspace launch");
 }
 
 // ---- Log (colorspace.c:1055-1163 forward, :2391-2500 inverse): a 65536-entry Quantum table indexed by ScaleQuantumToMap
@@ -692,44 +683,29 @@ __global__ void __launch_bounds__(256) ycc_leg_kernel(float *buf, size_t npixels
   else { q[0] = o[0]; q[1] = o[1]; q[2] = o[2]; }
 }
 
-// table (host, `entries` floats) -> stream-ordered device temporary -> gather kernel -> stream-ordered free
-template <typename Launch>
-int with_device_table(const float *host, size_t entries, cudaStream_t s, Launch &&launch) {
-  float *d = nullptr;
-  cudaError_t e = cudaMallocAsync(reinterpret_cast<void **>(&d), entries * sizeof(float), temp_pool(), s);
-  if (e != cudaSuccess) return cuda_fail(e, "colorspace: table allocation");
-  e = cudaMemcpyAsync(d, host, entries * sizeof(float), cudaMemcpyHostToDevice, s);     // pageable source: staged before return
-  int rc = e == cudaSuccess ? MB200_OK : cuda_fail(e, "colorspace: table upload");
-  if (rc == MB200_OK) {
-    launch(d);
-    count_launch();
-    e = cudaGetLastError();
-    if (e != cudaSuccess) rc = cuda_fail(e, "colorspace launch");
-  }
-  cudaFreeAsync(d, s);
-  return rc;
-}
-
 int launch_log_leg(float *buf, size_t npixels, int channels, bool forward, const mb200_colorspace_options *o, cudaStream_t s) {
-  const int rc = ensure_decode_scale();
+  int rc = ensure_decode_scale();
   if (rc) return rc;
   std::vector<float> table(65536);
   build_log_table(forward, o, table.data());
+  StreamAlloc d(s);
+  if ((rc = d.upload(table.data(), table.size() * sizeof(float), "colorspace: table upload"))) return rc;
   const unsigned blocks = static_cast<unsigned>((npixels + 255) / 256);
-  return with_device_table(table.data(), table.size(), s, [&](const float *d) {
-    if (channels == 4) log_leg_kernel<4><<<blocks, 256, 0, s>>>(buf, npixels, d, forward ? 1 : 0);
-    else log_leg_kernel<3><<<blocks, 256, 0, s>>>(buf, npixels, d, forward ? 1 : 0);
-  });
+  if (channels == 4) log_leg_kernel<4><<<blocks, 256, 0, s>>>(buf, npixels, d.as<float>(), forward ? 1 : 0);
+  else log_leg_kernel<3><<<blocks, 256, 0, s>>>(buf, npixels, d.as<float>(), forward ? 1 : 0);
+  return launch_status("colorspace launch");
 }
 
 int launch_ycc_leg(float *buf, size_t npixels, int channels, bool forward, cudaStream_t s) {
   float table[kYccEntries];
   build_ycc_table(table);
+  StreamAlloc d(s);
+  const int rc = d.upload(table, sizeof(table), "colorspace: table upload");
+  if (rc) return rc;
   const unsigned blocks = static_cast<unsigned>((npixels + 255) / 256);
-  return with_device_table(table, kYccEntries, s, [&](const float *d) {
-    if (channels == 4) ycc_leg_kernel<4><<<blocks, 256, 0, s>>>(buf, npixels, d, forward ? 1 : 0);
-    else ycc_leg_kernel<3><<<blocks, 256, 0, s>>>(buf, npixels, d, forward ? 1 : 0);
-  });
+  if (channels == 4) ycc_leg_kernel<4><<<blocks, 256, 0, s>>>(buf, npixels, d.as<float>(), forward ? 1 : 0);
+  else ycc_leg_kernel<3><<<blocks, 256, 0, s>>>(buf, npixels, d.as<float>(), forward ? 1 : 0);
+  return launch_status("colorspace launch");
 }
 
 }  // namespace
@@ -746,8 +722,7 @@ int launch_colorspace(float *buf, size_t npixels, int channels, int from, int to
   if (channels != 3 && channels != 4) return fail(MB200_EUNSUPPORTED, "colorspace: %d channels", channels);
   if (npixels == 0) return MB200_OK;
   if (npixels > 0xffffffffull * 256) return fail(MB200_EINVAL, "colorspace: image too large");
-  if (channels == 4 && (reinterpret_cast<uintptr_t>(buf) & 15) != 0)
-    return fail(MB200_EINVAL, "colorspace: RGBA buffers must be 16-byte aligned");
+  if (channels == 4 && !aligned16(buf)) return fail(MB200_EINVAL, "colorspace: RGBA buffers must be 16-byte aligned");
   if (options && (options->set & MB200_CO_ILLUMINANT) && (options->illuminant < 0 || options->illuminant > 10))
     return fail(MB200_EINVAL, "colorspace: illuminant %d", options->illuminant);
   cudaStream_t s = static_cast<cudaStream_t>(stream);

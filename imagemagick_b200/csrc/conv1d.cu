@@ -24,7 +24,7 @@
 //    float4 loads (odd pixel pitch => conflict-free LDS for the 8-rows x 4-channels
 //    lane layout).
 // No tensor cores: this is not a dense contraction.
-#include "mb200_internal.h"
+#include "launch.cuh"
 #include "conv_common.cuh"
 
 #include <cuda_runtime.h>
@@ -731,10 +731,7 @@ int launch_nt(const Conv1dArgs &base, int axis, const double *taps_host, int nta
     conv_row_kernel<NT, MODE, kMinBlocks><<<grid, 128, smem, stream>>>(a, taps);
     count_family(kConvGeneric);
   }
-  count_launch();
-  const cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return cuda_fail(e, "conv1d launch");
-  return MB200_OK;
+  return launch_status("conv1d launch");
 }
 
 template <int NT>

@@ -28,7 +28,7 @@
 // poison outputs the reference computes from finite samples only.  The loader therefore tests every sample's exponent
 // field and keeps one flag per 8-position block of the ring; an output block whose window holds a flagged block is
 // evaluated by a scalar DFMA loop over the window's own taps instead (rare: HDRI images with inf / NaN pixels).
-#include "mb200_internal.h"
+#include "launch.cuh"
 #include "conv_common.cuh"
 #include "tma.cuh"
 
@@ -728,12 +728,9 @@ int launch_wide(const MmaArgs &a, const double *taps_host, cudaStream_t stream) 
   const long long tiles = (lines + 7) / 8 * ((len + a.strip - 1) / a.strip);
   const int grid = static_cast<int>(std::min<long long>(static_cast<long long>(kCtasPerSm) * sm_count(), (tiles + 3) / 4));
   kernel<<<grid, 128, smem, stream>>>(a, taps, tmap);
-  count_launch();
   count_family(kConvMma);
   count_family(kConvMmaWide);
-  const cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return cuda_fail(e, "conv_mma_wide launch");
-  return MB200_OK;
+  return launch_status("conv_mma_wide launch");
 }
 
 template <int NKS>
@@ -758,11 +755,8 @@ int launch_one(const MmaArgs &a, const MmaTaps<NKS> &taps, int minb, cudaStream_
   };
   if (minb >= 4) go(conv_mma_kernel<NKS, AXIS, IO, EPI, 4>);
   else go(conv_mma_kernel<NKS, AXIS, IO, EPI, 3>);
-  count_launch();
   count_family(kConvMma);
-  const cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return cuda_fail(e, "conv_mma launch");
-  return MB200_OK;
+  return launch_status("conv_mma launch");
 }
 
 template <int NKS>

@@ -7,7 +7,7 @@
 // parameters; the 1024-entry weight table and every per-call value travel in a __grid_constant__ parameter, so a call
 // uploads nothing.  The reference's integer conversions are x86's: (ssize_t) / (int) of NaN or of an out-of-range value
 // is the most negative integer, which CUDA's saturating cvt would not give.
-#include "mb200_internal.h"
+#include "launch.cuh"
 #include "quantum.cuh"
 
 #include <climits>
@@ -392,8 +392,8 @@ int launch_distort(const float *src, size_t width, size_t height, int channels, 
   else if (persp) distort_kernel<true, false><<<grid, block, 0, s>>>(p, src, dst);
   else if (edge) distort_kernel<false, true><<<grid, block, 0, s>>>(p, src, dst);
   else distort_kernel<false, false><<<grid, block, 0, s>>>(p, src, dst);
-  const cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return cuda_fail(e, "distort launch");
+  rc = launch_status("distort launch", 0);
+  if (rc) return rc;
   count_family(kDistort);
   return MB200_OK;
 }

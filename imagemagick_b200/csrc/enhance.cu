@@ -11,14 +11,13 @@
 // Every operation whose result a branch depends on is the reference's own IEEE double operation in its order, unfused
 // (the hexcone.cuh legs, Polynomial, the Grayscale means); sin / asin / atan / atan2 / cos come from the CUDA math library
 // instead of glibc (<= 1 ULP of the float Quantum), as do the gamma curves and cube roots of colorspace_math.cuh.
-#include "mb200_internal.h"
+#include "launch.cuh"
 #include "colorspace_math.cuh"
 #include "hexcone.cuh"
 
 #include <cuda_runtime.h>
 
 #include <cmath>
-#include <cstdint>
 
 namespace mb200 {
 namespace {
@@ -261,52 +260,16 @@ __global__ void __launch_bounds__(256) function_kernel(float *buf, size_t npixel
   store_px<CH, VEC>(q, v);
 }
 
-// One launch of KERNEL<CH, VEC> over the image: float4 only for 16-byte aligned RGBA.
-template <template <int, bool> class K, typename... Args>
-int launch_point(const char *what, float *buf, size_t npixels, int channels, void *stream, Args... args) {
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  const unsigned blocks = static_cast<unsigned>((npixels + 255) / 256);
-  const bool vec = channels == 4 && (reinterpret_cast<uintptr_t>(buf) & 15) == 0;
-  switch (channels) {
-    case 1: K<1, false>::launch(blocks, s, buf, npixels, args...); break;
-    case 2: K<2, false>::launch(blocks, s, buf, npixels, args...); break;
-    case 3: K<3, false>::launch(blocks, s, buf, npixels, args...); break;
-    default:
-      if (vec) K<4, true>::launch(blocks, s, buf, npixels, args...);
-      else K<4, false>::launch(blocks, s, buf, npixels, args...);
-      break;
-  }
-  count_launch();
-  const cudaError_t e = cudaGetLastError();
-  return e == cudaSuccess ? MB200_OK : cuda_fail(e, what);
-}
-
-template <int CH, bool VEC> struct Contrast {
-  static void launch(unsigned blocks, cudaStream_t s, float *buf, size_t n, double half_sign) {
-    contrast_kernel<CH, VEC><<<blocks, 256, 0, s>>>(buf, n, half_sign);
-  }
-};
-template <int CH, bool VEC> struct Modulate {
-  static void launch(unsigned blocks, cudaStream_t s, float *buf, size_t n, ModulateArgs a) {
-    modulate_kernel<CH, VEC><<<blocks, 256, 0, s>>>(buf, n, a);
-  }
-};
-template <int CH, bool VEC> struct Grayscale {
-  static void launch(unsigned blocks, cudaStream_t s, float *buf, size_t n, int method, int gamma) {
-    grayscale_kernel<CH, VEC><<<blocks, 256, 0, s>>>(buf, n, method, gamma);
-  }
-};
-template <int CH, bool VEC> struct Function {
-  static void launch(unsigned blocks, cudaStream_t s, float *buf, size_t n, FunctionArgs a) {
-    function_kernel<CH, VEC><<<blocks, 256, 0, s>>>(buf, n, a);
-  }
-};
-
 }  // namespace
 
 int launch_contrast(float *buf, size_t npixels, int channels, bool sharpen, void *stream) {
   const double half_sign = 0.5 * (sharpen ? 1 : -1);
-  return launch_point<Contrast>("contrast launch", buf, npixels, channels, stream, half_sign);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const unsigned blocks = static_cast<unsigned>((npixels + 255) / 256);
+  return with_channels(channels, aligned16(buf), "contrast", [&](auto ch, auto vec) {
+    contrast_kernel<ch(), vec()><<<blocks, 256, 0, s>>>(buf, npixels, half_sign);
+    return launch_status("contrast launch");
+  });
 }
 
 int launch_modulate(float *buf, size_t npixels, int channels, double percent_brightness, double percent_saturation,
@@ -331,7 +294,12 @@ int launch_modulate(float *buf, size_t npixels, int channels, double percent_bri
   o.set = MB200_CO_ILLUMINANT;
   o.illuminant = illuminant;
   a.st = xyz_settings(&o);
-  return launch_point<Modulate>("modulate launch", buf, npixels, channels, stream, a);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const unsigned blocks = static_cast<unsigned>((npixels + 255) / 256);
+  return with_channels(channels, aligned16(buf), "modulate", [&](auto ch, auto vec) {
+    modulate_kernel<ch(), vec()><<<blocks, 256, 0, s>>>(buf, npixels, a);
+    return launch_status("modulate launch");
+  });
 }
 
 int launch_grayscale(float *buf, size_t npixels, int channels, int method, int image_colorspace, void *stream) {
@@ -342,7 +310,12 @@ int launch_grayscale(float *buf, size_t npixels, int channels, int method, int i
                     method == MB200_UndefinedPixelIntensityMethod;
   if (luma && image_colorspace == MB200_RGBColorspace) gamma = kEncode;
   if (luminance && image_colorspace == MB200_sRGBColorspace) gamma = kDecode;
-  return launch_point<Grayscale>("grayscale launch", buf, npixels, channels, stream, method, gamma);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const unsigned blocks = static_cast<unsigned>((npixels + 255) / 256);
+  return with_channels(channels, aligned16(buf), "grayscale", [&](auto ch, auto vec) {
+    grayscale_kernel<ch(), vec()><<<blocks, 256, 0, s>>>(buf, npixels, method, gamma);
+    return launch_status("grayscale launch");
+  });
 }
 
 int launch_function(float *buf, size_t npixels, int channels, int function, size_t n, const double *params,
@@ -352,7 +325,12 @@ int launch_function(float *buf, size_t npixels, int channels, int function, size
   a.n = static_cast<int>(n);
   a.function = function;
   a.update_mask = update_mask;
-  return launch_point<Function>("function launch", buf, npixels, channels, stream, a);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const unsigned blocks = static_cast<unsigned>((npixels + 255) / 256);
+  return with_channels(channels, aligned16(buf), "function", [&](auto ch, auto vec) {
+    function_kernel<ch(), vec()><<<blocks, 256, 0, s>>>(buf, npixels, a);
+    return launch_status("function launch");
+  });
 }
 
 }  // namespace mb200

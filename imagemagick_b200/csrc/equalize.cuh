@@ -1,6 +1,6 @@
-// equalize.cuh -- the histogram and table-apply kernels of EqualizeImage (equalize.cu), shared with the histogram-driven
-// level operators (level.cu: ContrastStretchImage, LinearStretchImage, GammaImage), which run the same two passes with a
-// table built on the host in between.
+// equalize.cuh -- the histogram and table-apply kernels of EqualizeImage and of the histogram-driven level operators
+// (level.cu: ContrastStretchImage, LinearStretchImage, GammaImage), which run the same two passes with a table built on
+// the host in between; AutoThresholdImage takes the histogram pass alone.
 #pragma once
 
 #include <cuda_runtime.h>

@@ -12,6 +12,7 @@
 // Structure: one thread per pixel, float4 access for RGBA, alpha untouched.  The six-sector fan-out of every inverse
 // transform is one permutation table (kSector) applied to the three values the sector formulae produce.
 #include "hexcone.cuh"
+#include "launch.cuh"
 
 #include <cuda_runtime.h>
 
@@ -66,10 +67,7 @@ int launch_hexcone_leg(float *buf, size_t npixels, int channels, int space, bool
   const unsigned blocks = static_cast<unsigned>((npixels + 255) / 256);
   if (channels == 4) hexcone_kernel<4><<<blocks, 256, 0, s>>>(buf, npixels, space, forward ? 1 : 0);
   else hexcone_kernel<3><<<blocks, 256, 0, s>>>(buf, npixels, space, forward ? 1 : 0);
-  count_launch();
-  const cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return cuda_fail(e, "hexcone launch");
-  return MB200_OK;
+  return launch_status("hexcone launch");
 }
 
 }  // namespace mb200

@@ -7,7 +7,7 @@
 // 8192^2 RGBA on one H100 80GB HBM3 at a 400 W power limit: Despeckle 20.2 ms (12.7 % of the 3.35 TB/s data-sheet HBM
 // bandwidth), LocalContrast 10x12.5 12.2 ms (23.6 % of the probed FP64 FMA rate), WaveletDenoise 10 % 11.7 ms (41 % of
 // HBM).
-#include "mb200_internal.h"
+#include "launch.cuh"
 
 #include <cuda_runtime.h>
 
@@ -15,11 +15,6 @@
 
 namespace mb200 {
 namespace {
-
-int launch_status(const char *what) {
-  const cudaError_t e = cudaGetLastError();
-  return e == cudaSuccess ? MB200_OK : cuda_fail(e, what);
-}
 
 // ------------------------------------------------------------------------------------------------------ DespeckleImage
 // The reference runs 16 Hulls per channel over a zero-bordered plane, each Hull two full-plane sweeps.  One launch here
@@ -314,18 +309,14 @@ int launch_despeckle(const float *src, float *dst, float *tmp, size_t w, size_t 
   // src -> tmp -> dst -> tmp -> dst: a launch never reads the buffer it writes (tiles read their neighbours' pixels)
   const float *in[4] = {src, tmp, dst, tmp};
   float *out[4] = {tmp, dst, tmp, dst};
-  for (int k = 0; k < 4; ++k) {
-    switch (channels) {
-      case 1: despeckle_kernel<1><<<grid, kDsThreads, 0, s>>>(in[k], out[k], iw, ih, X[k], Y[k]); break;
-      case 2: despeckle_kernel<2><<<grid, kDsThreads, 0, s>>>(in[k], out[k], iw, ih, X[k], Y[k]); break;
-      case 3: despeckle_kernel<3><<<grid, kDsThreads, 0, s>>>(in[k], out[k], iw, ih, X[k], Y[k]); break;
-      default: despeckle_kernel<4><<<grid, kDsThreads, 0, s>>>(in[k], out[k], iw, ih, X[k], Y[k]); break;
+  return with_channels(channels, "despeckle", [&](auto ch) -> int {
+    for (int k = 0; k < 4; ++k) {
+      despeckle_kernel<ch()><<<grid, kDsThreads, 0, s>>>(in[k], out[k], iw, ih, X[k], Y[k]);
+      const int rc = launch_status("despeckle launch");
+      if (rc) return rc;
     }
-    count_launch();
-    rc = launch_status("despeckle launch");
-    if (rc) return rc;
-  }
-  return MB200_OK;
+    return MB200_OK;
+  });
 }
 
 long local_contrast_width(size_t w, size_t h, double radius) {
@@ -357,27 +348,16 @@ int launch_local_contrast(const float *src, float *dst, float *luma, float *inte
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const size_t n = w * h;
   const unsigned lblocks = static_cast<unsigned>((n + 255) / 256);
-  switch (channels) {
-    case 1: luma_kernel<1><<<lblocks, 256, 0, s>>>(src, luma, n); break;
-    case 2: luma_kernel<2><<<lblocks, 256, 0, s>>>(src, luma, n); break;
-    case 3: luma_kernel<3><<<lblocks, 256, 0, s>>>(src, luma, n); break;
-    default: luma_kernel<4><<<lblocks, 256, 0, s>>>(src, luma, n); break;
-  }
-  count_launch();
   const int iw = static_cast<int>(w), ih = static_cast<int>(h);
   const dim3 vgrid(static_cast<unsigned>((w + 31) / 32), static_cast<unsigned>((h + kLcVRows - 1) / kLcVRows));
-  local_contrast_v_kernel<<<vgrid, dim3(32, kLcVThreadsY), 0, s>>>(luma, inter, iw, ih, width, total);
-  count_launch();
   const dim3 hgrid(static_cast<unsigned>((w + kLcHThreads * kLcHOut - 1) / (kLcHThreads * kLcHOut)), static_cast<unsigned>(h));
   const double strength100 = strength / 100.0;
-  switch (channels) {
-    case 1: local_contrast_h_kernel<1><<<hgrid, kLcHThreads, 0, s>>>(src, luma, inter, dst, iw, width, total, strength100); break;
-    case 2: local_contrast_h_kernel<2><<<hgrid, kLcHThreads, 0, s>>>(src, luma, inter, dst, iw, width, total, strength100); break;
-    case 3: local_contrast_h_kernel<3><<<hgrid, kLcHThreads, 0, s>>>(src, luma, inter, dst, iw, width, total, strength100); break;
-    default: local_contrast_h_kernel<4><<<hgrid, kLcHThreads, 0, s>>>(src, luma, inter, dst, iw, width, total, strength100); break;
-  }
-  count_launch();
-  return launch_status("local contrast launch");
+  return with_channels(channels, "local contrast", [&](auto ch) {
+    luma_kernel<ch()><<<lblocks, 256, 0, s>>>(src, luma, n);
+    local_contrast_v_kernel<<<vgrid, dim3(32, kLcVThreadsY), 0, s>>>(luma, inter, iw, ih, width, total);
+    local_contrast_h_kernel<ch()><<<hgrid, kLcHThreads, 0, s>>>(src, luma, inter, dst, iw, width, total, strength100);
+    return launch_status("local contrast launch", 3);
+  });
 }
 
 int wavelet_denoise_supported(size_t w, size_t h) {
@@ -409,7 +389,6 @@ int launch_wavelet_denoise(const float *src, float *dst, float *planes, size_t w
     lv.softness = static_cast<float>(softness);
     wavelet_level_kernel<<<grid, dim3(32, 8), 0, s>>>(src, dst, channels, low[(level + 1) & 1], low[level & 1], acc, iw,
                                                       ih, lv);
-    count_launch();
     rc = launch_status("wavelet denoise launch");
     if (rc) return rc;
   }

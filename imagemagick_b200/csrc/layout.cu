@@ -18,7 +18,7 @@
 // gamma steps are the colorspace_math.cuh curves with NaN / +inf settled like the reference's: <= 1 ULP.
 // One thread per pixel.  RGBA / CMYK (16 bytes) move as float4 and gray + alpha (8 bytes) as float2 when both buffers
 // are aligned for their widths; RGB, gray and CMYKA (20 bytes, never 16-byte aligned) move per channel.
-#include "mb200_internal.h"
+#include "launch.cuh"
 #include "colorspace_math.cuh"
 #include "hexcone.cuh"
 
@@ -111,8 +111,7 @@ __global__ void __launch_bounds__(256) layout_kernel(const float *__restrict__ s
 }
 
 bool aligned_for(const void *p, int channels) {
-  const uintptr_t a = reinterpret_cast<uintptr_t>(p);
-  return channels == 4 ? (a & 15) == 0 : channels == 2 ? (a & 7) == 0 : true;
+  return channels == 4 ? aligned16(p) : channels == 2 ? (reinterpret_cast<uintptr_t>(p) & 7) == 0 : true;
 }
 
 template <int LEG, bool ALPHA>
@@ -127,9 +126,7 @@ template <int LEG>
 int launch_leg(const float *src, float *dst, size_t npixels, bool alpha, cudaStream_t s) {
   if (alpha) launch_leg_as<LEG, true>(src, dst, npixels, s);
   else launch_leg_as<LEG, false>(src, dst, npixels, s);
-  count_launch();
-  const cudaError_t e = cudaGetLastError();
-  return e == cudaSuccess ? MB200_OK : cuda_fail(e, "colorspace layout launch");
+  return launch_status("colorspace layout launch");
 }
 
 // The layout leg between `cs` and sRGB (forward: sRGB -> cs).
@@ -141,20 +138,6 @@ int run_layout_leg(int cs, bool forward, const float *src, float *dst, size_t np
   return forward ? launch_leg<kToLinearGray>(src, dst, npixels, alpha, s)
                  : launch_leg<kFromLinearGray>(src, dst, npixels, alpha, s);
 }
-
-struct PoolBuffer {            // stream-ordered temporary from the library's pool, freed (stream-ordered) on scope exit
-  float *ptr = nullptr;
-  cudaStream_t s;
-  explicit PoolBuffer(cudaStream_t stream) : s(stream) {}
-  int alloc(size_t bytes) {
-    const cudaError_t e = cudaMallocAsync(reinterpret_cast<void **>(&ptr), bytes, temp_pool(), s);
-    if (e != cudaSuccess) { ptr = nullptr; return cuda_fail(e, "colorspace layout: temporary"); }
-    return MB200_OK;
-  }
-  ~PoolBuffer() { if (ptr) cudaFreeAsync(ptr, s); }
-  PoolBuffer(const PoolBuffer &) = delete;
-  PoolBuffer &operator=(const PoolBuffer &) = delete;
-};
 
 }  // namespace
 
@@ -190,13 +173,13 @@ int launch_colorspace_layout(const float *src, int src_channels, float *dst, int
   // `work` holds the image in sRGB between the two legs: dst itself when the target is a 3/4-channel space whose
   // in-place leg can run there (3 channels, or RGBA on a 16-byte boundary), a temporary otherwise
   const bool work_is_dst = !to_layout && (rgb_channels == 3 || aligned_for(dst, 4));
-  PoolBuffer tmp(s);
+  StreamAlloc tmp(s);
   float *work = dst;
   int rc = MB200_OK;
   if (!work_is_dst) {
-    rc = tmp.alloc(rgb_bytes);
+    rc = tmp.alloc(rgb_bytes, "colorspace layout: temporary");
     if (rc) return rc;
-    work = tmp.ptr;
+    work = tmp.as<float>();
   }
   if (from_layout) {
     rc = run_layout_leg(from, false, src, work, npixels, alpha, s);

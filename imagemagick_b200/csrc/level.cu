@@ -18,11 +18,21 @@
 // level kernel takes the reference's fabs(min-max) >= MagickEpsilon decision itself, so nothing is read back.  Ties of
 // +0 and -0 are resolved in no particular order, as the reference's parallel row merge resolves them.
 //
+// EqualizeImage (enhance.c:2040-2290; also the second half of EmbossImage, effect.c:1600-1681):
+//   1. histogram[bin][i]++ for every channel i of every pixel, bin = ScaleQuantumToMap(ClampToQuantum(intensity)) where
+//      intensity is the pixel's GetPixelIntensity (Rec709 luma; the gray sample of gray images) when the channel mask
+//      carries SyncChannels -- which the default mask (AllChannels) does -- and the channel's own value otherwise (:2125-2129);
+//   2. map = running sum of the histogram; black = map[0], white = map[MaxMap];
+//      equalize_map[j] = ScaleMapToQuantum(MaxMap * (map[j] - black) / (white - black))              (:2138-2169)
+//   3. every channel with black != white: q = equalize_map[ScaleQuantumToMap(q)]                      (:2229-2260)
+// Steps 1 and 3 are the two passes of equalize.cuh (integer counts: exact; table lookup: exact), step 2 -- 65 536 doubles
+// per channel in the reference's own order -- runs on the host between them, so the result is bit-identical.
+//
 // ContrastStretch, LinearStretch and Gamma are EqualizeImage's two passes (equalize.cuh: histogram, table apply) with
 // their own table, built on the host in the reference's order; ContrastStretch and LinearStretch read the histogram back
 // (the stream is synchronised).  Gamma reads nothing back, but its table is a pageable upload, which CUDA orders after
 // the stream's earlier work.
-#include "mb200_internal.h"
+#include "launch.cuh"
 #include "equalize.cuh"
 #include "quantum.cuh"
 
@@ -30,7 +40,6 @@
 
 #include <cmath>
 #include <algorithm>
-#include <cstdint>
 #include <vector>
 
 namespace mb200 {
@@ -190,31 +199,14 @@ __global__ void __launch_bounds__(256) gray_kernel(const float *__restrict__ buf
   if ((threadIdx.x & 31) == 0 && f) atomicOr(flags, f);
 }
 
-bool rgba_vec(const float *buf, int channels) { return channels == 4 && (reinterpret_cast<uintptr_t>(buf) & 15) == 0; }
-
-int grid_of(size_t n, unsigned block, unsigned *grid, const char *what) {
-  const size_t blocks = (n + block - 1) / block;
-  if (blocks == 0 || blocks > 0x7fffffffull) return fail(MB200_EINVAL, "%s: bad image size", what);
-  *grid = static_cast<unsigned>(blocks);
-  return MB200_OK;
-}
-
 int launch_level_pass(float *buf, size_t npixels, int channels, const LevelArgs &a, cudaStream_t s) {
   unsigned grid;
   int rc = grid_of(npixels, 256, &grid, "level");
   if (rc) return rc;
-  switch (channels) {
-    case 1: level_kernel<1, false><<<grid, 256, 0, s>>>(buf, npixels, a); break;
-    case 2: level_kernel<2, false><<<grid, 256, 0, s>>>(buf, npixels, a); break;
-    case 3: level_kernel<3, false><<<grid, 256, 0, s>>>(buf, npixels, a); break;
-    default:
-      if (rgba_vec(buf, channels)) level_kernel<4, true><<<grid, 256, 0, s>>>(buf, npixels, a);
-      else level_kernel<4, false><<<grid, 256, 0, s>>>(buf, npixels, a);
-      break;
-  }
-  count_launch();
-  const cudaError_t e = cudaGetLastError();
-  return e == cudaSuccess ? MB200_OK : cuda_fail(e, "level launch");
+  return with_channels(channels, aligned16(buf), "level", [&](auto ch, auto vec) {
+    level_kernel<ch(), vec()><<<grid, 256, 0, s>>>(buf, npixels, a);
+    return launch_status("level launch");
+  });
 }
 
 // GetImageRange over the channels of `select` into range[0..1] (rows: 2 * height doubles of scratch)
@@ -222,31 +214,11 @@ int launch_range(const float *buf, size_t width, size_t height, int channels, un
                  cudaStream_t s) {
   if (height == 0 || height > 0x7fffffffull) return fail(MB200_EINVAL, "range: bad image size");
   const unsigned grid = static_cast<unsigned>(height);
-  switch (channels) {
-    case 1: range_rows_kernel<1, false><<<grid, 256, 0, s>>>(buf, width, select, rows); break;
-    case 2: range_rows_kernel<2, false><<<grid, 256, 0, s>>>(buf, width, select, rows); break;
-    case 3: range_rows_kernel<3, false><<<grid, 256, 0, s>>>(buf, width, select, rows); break;
-    default:
-      if (rgba_vec(buf, channels)) range_rows_kernel<4, true><<<grid, 256, 0, s>>>(buf, width, select, rows);
-      else range_rows_kernel<4, false><<<grid, 256, 0, s>>>(buf, width, select, rows);
-      break;
-  }
-  count_launch();
-  range_merge_kernel<<<1, 1024, 0, s>>>(rows, height, range);
-  count_launch();
-  const cudaError_t e = cudaGetLastError();
-  return e == cudaSuccess ? MB200_OK : cuda_fail(e, "range launch");
-}
-
-template <bool CHAR_BINS>
-void launch_histogram(const float *buf, size_t npixels, int channels, int sync, unsigned *d_counts, unsigned grid,
-                      cudaStream_t s) {
-  switch (channels) {
-    case 1: histogram_kernel<1, CHAR_BINS><<<grid, 256, 0, s>>>(buf, npixels, sync, d_counts); break;
-    case 2: histogram_kernel<2, CHAR_BINS><<<grid, 256, 0, s>>>(buf, npixels, sync, d_counts); break;
-    case 3: histogram_kernel<3, CHAR_BINS><<<grid, 256, 0, s>>>(buf, npixels, sync, d_counts); break;
-    default: histogram_kernel<4, CHAR_BINS><<<grid, 256, 0, s>>>(buf, npixels, sync, d_counts); break;
-  }
+  return with_channels(channels, aligned16(buf), "range", [&](auto ch, auto vec) {
+    range_rows_kernel<ch(), vec()><<<grid, 256, 0, s>>>(buf, width, select, rows);
+    range_merge_kernel<<<1, 1024, 0, s>>>(rows, height, range);
+    return launch_status("range launch", 2);
+  });
 }
 
 // The histogram pass of equalize.cuh into a fresh device buffer of nhist * kBins counts, read back into `counts`;
@@ -258,21 +230,19 @@ int histogram_readback(const float *buf, size_t npixels, int channels, int sync,
   if (rc) return rc;
   if (char_bins) sync = 1;
   const int nhist = sync ? 1 : channels;
-  unsigned *d_counts = nullptr;
-  cudaError_t e = cudaMallocAsync(reinterpret_cast<void **>(&d_counts), sizeof(unsigned) * kBins * nhist, temp_pool(), s);
-  if (e != cudaSuccess) return cuda_fail(e, "histogram: allocation");
-  e = cudaMemsetAsync(d_counts, 0, sizeof(unsigned) * kBins * nhist, s);
-  if (e == cudaSuccess) {
-    if (char_bins) launch_histogram<true>(buf, npixels, channels, sync, d_counts, grid, s);
-    else launch_histogram<false>(buf, npixels, channels, sync, d_counts, grid, s);
-    count_launch();
-    counts->assign(static_cast<size_t>(kBins) * nhist, 0u);
-    e = cudaGetLastError();
-  }
-  if (e == cudaSuccess)
-    e = cudaMemcpyAsync(counts->data(), d_counts, counts->size() * sizeof(unsigned), cudaMemcpyDeviceToHost, s);
+  StreamAlloc d_counts(s);
+  if ((rc = d_counts.alloc(sizeof(unsigned) * kBins * nhist, "histogram: allocation"))) return rc;
+  cudaError_t e = cudaMemsetAsync(d_counts.ptr, 0, sizeof(unsigned) * kBins * nhist, s);
+  if (e != cudaSuccess) return cuda_fail(e, "histogram readback");
+  rc = with_channels(channels, "histogram", [&](auto ch) {
+    if (char_bins) histogram_kernel<ch(), true><<<grid, 256, 0, s>>>(buf, npixels, sync, d_counts.as<unsigned>());
+    else histogram_kernel<ch(), false><<<grid, 256, 0, s>>>(buf, npixels, sync, d_counts.as<unsigned>());
+    return launch_status("histogram readback");
+  });
+  if (rc) return rc;
+  counts->assign(static_cast<size_t>(kBins) * nhist, 0u);
+  e = cudaMemcpyAsync(counts->data(), d_counts.ptr, counts->size() * sizeof(unsigned), cudaMemcpyDeviceToHost, s);
   if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-  cudaFreeAsync(d_counts, s);
   return e == cudaSuccess ? MB200_OK : cuda_fail(e, "histogram readback");
 }
 
@@ -284,23 +254,13 @@ int apply_table(float *buf, size_t npixels, int channels, const std::vector<floa
   unsigned grid;
   int rc = grid_of(npixels, 256, &grid, "table");
   if (rc) return rc;
-  float *d_table = nullptr;
-  cudaError_t e = cudaMallocAsync(reinterpret_cast<void **>(&d_table), table.size() * sizeof(float), temp_pool(), s);
-  if (e != cudaSuccess) return cuda_fail(e, "table: allocation");
-  rc = copy_h2d(d_table, table.data(), table.size() * sizeof(float), s);
-  if (!rc) {
-    switch (channels) {
-      case 1: equalize_apply_kernel<1><<<grid, 256, 0, s>>>(buf, npixels, d_table, enabled); break;
-      case 2: equalize_apply_kernel<2><<<grid, 256, 0, s>>>(buf, npixels, d_table, enabled); break;
-      case 3: equalize_apply_kernel<3><<<grid, 256, 0, s>>>(buf, npixels, d_table, enabled); break;
-      default: equalize_apply_kernel<4><<<grid, 256, 0, s>>>(buf, npixels, d_table, enabled); break;
-    }
-    count_launch();
-    e = cudaGetLastError();
-    if (e != cudaSuccess) rc = cuda_fail(e, "table launch");
-  }
-  cudaFreeAsync(d_table, s);
-  return rc;
+  StreamAlloc d_table(s);
+  if ((rc = d_table.alloc(table.size() * sizeof(float), "table: allocation"))) return rc;
+  if ((rc = copy_h2d(d_table.ptr, table.data(), table.size() * sizeof(float), s))) return rc;
+  return with_channels(channels, "table", [&](auto ch) {
+    equalize_apply_kernel<ch()><<<grid, 256, 0, s>>>(buf, npixels, d_table.as<float>(), enabled);
+    return launch_status("table launch");
+  });
 }
 
 // ScaleMapToQuantum (quantum-private.h:465-475, HDRI)
@@ -327,16 +287,15 @@ int launch_level(float *buf, size_t npixels, int channels, double black, double 
 int launch_minmax_stretch(float *buf, size_t width, size_t height, int channels, double black, double white, double gamma,
                           bool per_channel, unsigned update_mask, void *stream) {
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  double *d_rows = nullptr;
-  cudaError_t e = cudaMallocAsync(reinterpret_cast<void **>(&d_rows), sizeof(double) * 2 * (height + 1), temp_pool(), s);
-  if (e != cudaSuccess) return cuda_fail(e, "minmax stretch: allocation");
-  double *d_range = d_rows + 2 * height;
+  StreamAlloc rows(s);
+  int rc = rows.alloc(sizeof(double) * 2 * (height + 1), "minmax stretch: allocation");
+  if (rc) return rc;
+  double *d_rows = rows.as<double>(), *d_range = d_rows + 2 * height;
   LevelArgs a{};
   a.black = black;
   a.white = white;
   a.exponent = perceptible_reciprocal(gamma);
   a.range = d_range;
-  int rc = MB200_OK;
   if (!per_channel) {                                            // histogram.c:944-953: all channels at once
     rc = launch_range(buf, width, height, channels, update_mask, d_rows, d_range, s);
     a.update_mask = update_mask;
@@ -353,7 +312,6 @@ int launch_minmax_stretch(float *buf, size_t width, size_t height, int channels,
       if (!rc) rc = launch_level_pass(buf, width * height, channels, a, s);
     }
   }
-  cudaFreeAsync(d_rows, s);
   return rc;
 }
 
@@ -440,24 +398,18 @@ int launch_identify_gray(const float *buf, size_t npixels, int channels, int *ty
   unsigned grid;
   int rc = grid_of(npixels, 256, &grid, "identify gray");
   if (rc) return rc;
-  unsigned *d_flags = nullptr;
-  cudaError_t e = cudaMallocAsync(reinterpret_cast<void **>(&d_flags), sizeof(unsigned), temp_pool(), s);
-  if (e != cudaSuccess) return cuda_fail(e, "identify gray: allocation");
-  e = cudaMemsetAsync(d_flags, 0, sizeof(unsigned), s);
-  if (e == cudaSuccess) {
-    switch (channels) {
-      case 1: gray_kernel<1><<<grid, 256, 0, s>>>(buf, npixels, d_flags); break;
-      case 2: gray_kernel<2><<<grid, 256, 0, s>>>(buf, npixels, d_flags); break;
-      case 3: gray_kernel<3><<<grid, 256, 0, s>>>(buf, npixels, d_flags); break;
-      default: gray_kernel<4><<<grid, 256, 0, s>>>(buf, npixels, d_flags); break;
-    }
-    count_launch();
-    e = cudaGetLastError();
-  }
+  StreamAlloc d_flags(s);
+  if ((rc = d_flags.alloc(sizeof(unsigned), "identify gray: allocation"))) return rc;
+  cudaError_t e = cudaMemsetAsync(d_flags.ptr, 0, sizeof(unsigned), s);
+  if (e != cudaSuccess) return cuda_fail(e, "identify gray");
+  rc = with_channels(channels, "identify gray", [&](auto ch) {
+    gray_kernel<ch()><<<grid, 256, 0, s>>>(buf, npixels, d_flags.as<unsigned>());
+    return launch_status("identify gray");
+  });
+  if (rc) return rc;
   unsigned flags = 0;
-  if (e == cudaSuccess) e = cudaMemcpyAsync(&flags, d_flags, sizeof(unsigned), cudaMemcpyDeviceToHost, s);
+  e = cudaMemcpyAsync(&flags, d_flags.ptr, sizeof(unsigned), cudaMemcpyDeviceToHost, s);
   if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-  cudaFreeAsync(d_flags, s);
   if (e != cudaSuccess) return cuda_fail(e, "identify gray");
   *type = (flags & 1u) ? 0 : (flags & 2u) ? 1 : 2;
   return MB200_OK;
@@ -469,6 +421,32 @@ int auto_threshold_histogram(const float *buf, size_t npixels, int channels, uns
   if (rc) return rc;
   std::copy(all.begin(), all.begin() + 256, counts);
   return MB200_OK;
+}
+
+int launch_equalize(float *buf, size_t npixels, int channels, int sync_channels, void *stream) {
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (channels < 1 || channels > 4) return fail(MB200_EINVAL, "equalize: 1..4 channels");
+  unsigned grid;
+  int rc = grid_of(npixels, 256, &grid, "equalize");
+  if (rc) return rc;
+  std::vector<unsigned> counts;
+  rc = histogram_readback(buf, npixels, channels, sync_channels, &counts, s);
+  if (rc) return rc;
+  // enhance.c:2138-2169 in the reference's order (running sums in double; 65 536 entries per channel)
+  std::vector<float> table(static_cast<size_t>(kBins) * channels, 0.0f);
+  unsigned enabled = 0;
+  for (int c = 0; c < channels; ++c) {
+    const unsigned *h = counts.data() + static_cast<size_t>(sync_channels ? 0 : c) * kBins;
+    std::vector<double> map(kBins);
+    double intensity = 0.0;
+    for (unsigned j = 0; j < kBins; ++j) { intensity += static_cast<double>(h[j]); map[j] = intensity; }
+    const double black = map[0], white = map[kBins - 1];
+    if (black == white) continue;
+    enabled |= 1u << c;
+    for (unsigned j = 0; j < kBins; ++j)
+      table[static_cast<size_t>(c) * kBins + j] = scale_map_to_quantum((65535.0 * (map[j] - black)) / (white - black));
+  }
+  return apply_table(buf, npixels, channels, table, enabled, s);
 }
 
 }  // namespace mb200

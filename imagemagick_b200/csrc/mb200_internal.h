@@ -270,7 +270,7 @@ int launch_scale(const float *src, size_t w, size_t h, int channels, float *dst,
 // SampleImage (resize.c:3907): nearest-sample gather, bit exact
 int launch_sample(const float *src, size_t w, size_t h, int channels, float *dst, size_t ow, size_t oh, void *stream);
 
-// equalize.cu: EqualizeImage (enhance.c:2040) in place; sync_channels = the channel mask carries SyncChannels (the
+// level.cu: EqualizeImage (enhance.c:2040) in place; sync_channels = the channel mask carries SyncChannels (the
 // default): one intensity-driven histogram for all channels.  Synchronises the stream (host step between the kernels).
 int launch_equalize(float *buf, size_t npixels, int channels, int sync_channels, void *stream);
 

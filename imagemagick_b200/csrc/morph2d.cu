@@ -13,7 +13,7 @@
 // in shared memory with coalesced loads; taps are read from a small global table
 // with warp-uniform (broadcast) loads; the active-cell list is compacted on the host so
 // NaN cells cost nothing.  Convolution accumulates in FP64.
-#include "mb200_internal.h"
+#include "launch.cuh"
 
 #include <cuda_runtime.h>
 
@@ -451,6 +451,13 @@ __global__ void __launch_bounds__(256) conv2d_dense_kernel(const Morph2dArgs a, 
   if (a.changed != nullptr && nchanged != 0) atomicAdd(a.changed, static_cast<unsigned long long>(nchanged));
 }
 
+// Raises the kernel's dynamic shared-memory limit to 200 KB (a per-device attribute), then launches it.
+template <typename... Params, typename... Args>
+void launch_large_smem(void (*kernel)(Params...), dim3 grid, dim3 block, size_t smem, cudaStream_t s, Args... args) {
+  cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+  kernel<<<grid, block, smem, s>>>(args...);
+}
+
 }  // namespace
 
 int launch_morph2d(const float *src, float *dst, size_t width, size_t height, int channels, int method,
@@ -481,7 +488,7 @@ int launch_morph2d(const float *src, float *dst, size_t width, size_t height, in
       host[n].du = static_cast<short>(u); host[n].dv = static_cast<short>(v); host[n].pad = 0.f; host[n].k = kept;
       ++n;
     }
-  const bool aligned = ((reinterpret_cast<uintptr_t>(src) | reinterpret_cast<uintptr_t>(dst)) & 15) == 0;
+  const bool aligned = aligned16(src, dst);
   if (method == MB200_ConvolveMorphology && n == total && aligned) {
     // every cell is part of the neighbourhood: register-tiled dense kernel (R = 8 or 4 output rows per thread while the
     // staged tile of doubles leaves room for two CTAs per SM, else 2 while it fits at all).  The conv2d_rows option
@@ -494,11 +501,9 @@ int launch_morph2d(const float *src, float *dst, size_t width, size_t height, in
     int R = tile_bytes(8) <= 110 * 1024 ? 8 : tile_bytes(4) <= 110 * 1024 ? 4 : (tile_bytes(2) <= 200 * 1024 ? 2 : 0);
     if (forced != 0 && tile_bytes(forced) <= 200 * 1024) R = forced;
     if (R != 0) {
-      double *d_taps = nullptr;
-      cudaError_t e = cudaMallocAsync(reinterpret_cast<void **>(&d_taps), sizeof(double) * static_cast<size_t>(total), temp_pool(), s);
-      if (e != cudaSuccess) return cuda_fail(e, "conv2d: tap table alloc");
-      e = cudaMemcpyAsync(d_taps, kernel_window_order, sizeof(double) * static_cast<size_t>(total), cudaMemcpyHostToDevice, s);
-      if (e != cudaSuccess) { cudaFreeAsync(d_taps, s); return cuda_fail(e, "conv2d: tap upload"); }
+      StreamAlloc taps(s);
+      const int rc = taps.upload(kernel_window_order, sizeof(double) * static_cast<size_t>(total), "conv2d: tap upload");
+      if (rc) return rc;
       Morph2dArgs a{};
       a.src = src; a.dst = dst;
       a.width = static_cast<int>(width); a.height = static_cast<int>(height); a.channels = channels;
@@ -506,32 +511,16 @@ int launch_morph2d(const float *src, float *dst, size_t width, size_t height, in
       a.bias = bias; a.gamma_scale = gamma_scale; a.method = method; a.changed = d_changed;
       const size_t smem = tile_bytes(R);
       dim3 grid((a.width + 31) / 32, (a.height + 8 * R - 1) / (8 * R)), block(32, 8);
-#define MB200_DENSE(CH, RR)                                                                                         \
-      do {                                                                                                          \
-        cudaFuncSetAttribute(conv2d_dense_kernel<CH, RR>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024); \
-        conv2d_dense_kernel<CH, RR><<<grid, block, smem, s>>>(a, d_taps);                                           \
-      } while (0)
-      switch (channels * 10 + R) {
-        case 18: MB200_DENSE(1, 8); break;
-        case 14: MB200_DENSE(1, 4); break;
-        case 12: MB200_DENSE(1, 2); break;
-        case 28: MB200_DENSE(2, 8); break;
-        case 24: MB200_DENSE(2, 4); break;
-        case 22: MB200_DENSE(2, 2); break;
-        case 38: MB200_DENSE(3, 8); break;
-        case 34: MB200_DENSE(3, 4); break;
-        case 32: MB200_DENSE(3, 2); break;
-        case 48: MB200_DENSE(4, 8); break;
-        case 44: MB200_DENSE(4, 4); break;
-        default: MB200_DENSE(4, 2); break;
-      }
-#undef MB200_DENSE
-      count_launch();
-      count_family(R == 8 ? kConv2dDenseR8 : R == 4 ? kConv2dDenseR4 : kConv2dDenseR2);
-      e = cudaGetLastError();
-      cudaFreeAsync(d_taps, s);
-      if (e != cudaSuccess) return cuda_fail(e, "conv2d launch");
-      return MB200_OK;
+      const double *d_taps = taps.as<const double>();
+      return with_channels(channels, "conv2d", [&](auto ch) {
+        switch (R) {
+          case 8: launch_large_smem(conv2d_dense_kernel<ch(), 8>, grid, block, smem, s, a, d_taps); break;
+          case 4: launch_large_smem(conv2d_dense_kernel<ch(), 4>, grid, block, smem, s, a, d_taps); break;
+          default: launch_large_smem(conv2d_dense_kernel<ch(), 2>, grid, block, smem, s, a, d_taps); break;
+        }
+        count_family(R == 8 ? kConv2dDenseR8 : R == 4 ? kConv2dDenseR4 : kConv2dDenseR2);
+        return launch_status("conv2d launch");
+      });
     }
     host = static_cast<Cell *>(malloc(sizeof(Cell) * static_cast<size_t>(total)));      // too large: the compacted-cell kernel
     if (!host) return fail(MB200_ENOMEM, "morph2d: host alloc");
@@ -543,18 +532,16 @@ int launch_morph2d(const float *src, float *dst, size_t width, size_t height, in
         ++n;
       }
   }
-  void *d_cells = nullptr;
-  cudaError_t e = cudaMallocAsync(&d_cells, sizeof(Cell) * static_cast<size_t>(total), temp_pool(), s);   // stream-ordered: re-entrant
-  if (e != cudaSuccess) { free(host); return cuda_fail(e, "morph2d: tap table alloc"); }
-  e = cudaMemcpyAsync(d_cells, host, sizeof(Cell) * static_cast<size_t>(n), cudaMemcpyHostToDevice, s);
-  free(host);   // pageable source: the copy has been staged when the call returns
-  if (e != cudaSuccess) { cudaFreeAsync(d_cells, s); return cuda_fail(e, "morph2d: tap upload"); }
+  StreamAlloc d_cells(s);                   // stream-ordered: re-entrant
+  const int rc = d_cells.upload(host, sizeof(Cell) * static_cast<size_t>(n), "morph2d: tap upload");
+  free(host);                               // pageable source: the copy has been staged when the call returns
+  if (rc) return rc;
 
   Morph2dArgs a{};
   a.src = src; a.dst = dst;
   a.width = static_cast<int>(width); a.height = static_cast<int>(height); a.channels = channels;
   a.ox = ox; a.oy = oy; a.kw = kw; a.kh = kh; a.ncells = n;
-  a.cells = static_cast<const Cell *>(d_cells);
+  a.cells = d_cells.as<const Cell>();
   a.bias = bias; a.gamma_scale = gamma_scale; a.method = method; a.changed = d_changed;
   if ((method == MB200_ErodeMorphology || method == MB200_DilateMorphology) && n <= 1024 && kw <= kMmPitch - kMmTile + 1 &&
       (channels != 4 || aligned)) {         // RGBA moves float4 pixels: unaligned buffers take morph2d_kernel below
@@ -563,52 +550,22 @@ int launch_morph2d(const float *src, float *dst, size_t width, size_t height, in
     if (msmem <= 160 * 1024) {
       dim3 mgrid((a.width + kMmTile - 1) / kMmTile, (a.height + kMmTile - 1) / kMmTile), mblock(32, 8);
       const bool dil = method == MB200_DilateMorphology;
-#define MB200_MM(CH)                                                                                   \
-      do {                                                                                             \
-        if (dil) {                                                                                     \
-          cudaFuncSetAttribute(minmax2d_kernel<CH, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);  \
-          minmax2d_kernel<CH, true><<<mgrid, mblock, msmem, s>>>(a);                            \
-        } else {                                                                                       \
-          cudaFuncSetAttribute(minmax2d_kernel<CH, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024); \
-          minmax2d_kernel<CH, false><<<mgrid, mblock, msmem, s>>>(a);                           \
-        }                                                                                              \
-      } while (0)
-      switch (channels) {
-        case 1: MB200_MM(1); break;
-        case 2: MB200_MM(2); break;
-        case 3: MB200_MM(3); break;
-        default: MB200_MM(4); break;
-      }
-#undef MB200_MM
-      count_launch();
-      count_family(kMinmax2d);
-      e = cudaGetLastError();
-      cudaFreeAsync(d_cells, s);
-      if (e != cudaSuccess) return cuda_fail(e, "minmax2d launch");
-      return MB200_OK;
+      return with_channels(channels, "minmax2d", [&](auto ch) {
+        if (dil) launch_large_smem(minmax2d_kernel<ch(), true>, mgrid, mblock, msmem, s, a);
+        else launch_large_smem(minmax2d_kernel<ch(), false>, mgrid, mblock, msmem, s, a);
+        count_family(kMinmax2d);
+        return launch_status("minmax2d launch");
+      });
     }
   }
   const size_t smem = static_cast<size_t>(kTileW + kw - 1) * (kTileH + kh - 1) * channels * sizeof(float);
-  if (smem > 200 * 1024) { cudaFreeAsync(d_cells, s); return fail(MB200_EUNSUPPORTED, "morph2d: %dx%d kernel needs %zu bytes of shared memory", kw, kh, smem); }
+  if (smem > 200 * 1024) return fail(MB200_EUNSUPPORTED, "morph2d: %dx%d kernel needs %zu bytes of shared memory", kw, kh, smem);
   dim3 grid((a.width + kTileW - 1) / kTileW, (a.height + kTileH - 1) / kTileH), block(kTileW, kTileH);
-#define MB200_LAUNCH(CH)                                                                         \
-  do {                                                                                           \
-    cudaFuncSetAttribute(morph2d_kernel<CH>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024); \
-    morph2d_kernel<CH><<<grid, block, smem, s>>>(a);                                             \
-  } while (0)
-  switch (channels) {
-    case 1: MB200_LAUNCH(1); break;
-    case 2: MB200_LAUNCH(2); break;
-    case 3: MB200_LAUNCH(3); break;
-    default: MB200_LAUNCH(4); break;
-  }
-#undef MB200_LAUNCH
-  count_launch();
-  count_family(kMorph2d);
-  e = cudaGetLastError();
-  cudaFreeAsync(d_cells, s);
-  if (e != cudaSuccess) return cuda_fail(e, "morph2d launch");
-  return MB200_OK;
+  return with_channels(channels, "morph2d", [&](auto ch) {
+    launch_large_smem(morph2d_kernel<ch()>, grid, block, smem, s, a);
+    count_family(kMorph2d);
+    return launch_status("morph2d launch");
+  });
 }
 
 }  // namespace mb200

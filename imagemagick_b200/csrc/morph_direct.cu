@@ -33,7 +33,7 @@
 // Voronoi on an image with alpha skips the alpha sweep; the reverse launch writes the epilogue instead (SetImageAlpha-
 // Channel(Deactivate), CompositeImage(CopyAlpha), Deactivate): alpha = ClampPixel(QuantumRange*(QuantumScale*a)) of the
 // source, every swept channel ClampPixel(value) (composite.c:2606-2612, :2708, :2860-2863, :3562).
-#include "mb200_internal.h"
+#include "launch.cuh"
 
 #include <cuda_runtime.h>
 
@@ -267,12 +267,12 @@ int launch_morphology_direct(const float *src, float *tmp, float *dst, size_t wi
   // one device block, zeroed on the stream before the launches: [tickets 2][progress 2 * nswept * nbands]
   const size_t nprog = static_cast<size_t>(nswept) * nbands;
   const size_t sync_bytes = (2 + 2 * nprog) * sizeof(int);
-  void *block = nullptr;
-  cudaError_t e = cudaMallocAsync(&block, sync_bytes, temp_pool(), s);
-  if (e != cudaSuccess) return cuda_fail(e, "morphology direct: cudaMallocAsync");
-  unsigned char *base = static_cast<unsigned char *>(block);
-  e = cudaMemsetAsync(base, 0, sync_bytes, s);
-  int rc = e == cudaSuccess ? MB200_OK : cuda_fail(e, "morphology direct: memset");
+  StreamAlloc block(s);
+  int rc = block.alloc(sync_bytes, "morphology direct: allocation");
+  if (rc) return rc;
+  unsigned char *base = block.as<unsigned char>();
+  cudaError_t e = cudaMemsetAsync(base, 0, sync_bytes, s);
+  if (e != cudaSuccess) rc = cuda_fail(e, "morphology direct: memset");
   static DirectArgs args[2];                            // 16 KB each: kept off the stack
   static std::mutex args_lock;
   std::lock_guard<std::mutex> lock(args_lock);          // the launch copies the parameters; the lock covers the staging
@@ -298,12 +298,10 @@ int launch_morphology_direct(const float *src, float *tmp, float *dst, size_t wi
     const unsigned grid = static_cast<unsigned>(nprog + (a.epilogue ? nbands : 0));
     if (rev) direct_sweep_kernel<true><<<grid, kBand, p.smem, s>>>(a);
     else direct_sweep_kernel<false><<<grid, kBand, p.smem, s>>>(a);
-    e = cudaGetLastError();
-    if (e != cudaSuccess) { rc = cuda_fail(e, "morphology direct: launch"); break; }
-    count_launch();
+    if ((rc = launch_status("morphology direct: launch", 0))) break;
+    count_launch();                                     // counted once the launch is known to have been accepted
     count_family(kMorphDirect);
   }
-  cudaFreeAsync(block, s);
   return rc;
 }
 

@@ -5,7 +5,7 @@
 // applied to every channel (all carry the Update trait on the accelerated path).
 //
 // threshold point operators of MagickCore/threshold.c (see threshold_kernel below).
-#include "mb200_internal.h"
+#include "launch.cuh"
 #include "conv_common.cuh"
 
 #include <cuda_runtime.h>
@@ -265,21 +265,11 @@ int launch_motion_blur(const float *src, float *dst, size_t w, size_t h, int cha
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   dim3 grid(static_cast<unsigned>((w + 127) / 128), static_cast<unsigned>(h));
   const int W = static_cast<int>(w), H = static_cast<int>(h);
-  switch (channels) {
-    case 1: motion_blur_kernel<1><<<grid, 128, 0, s>>>(src, dst, W, H, a); break;
-    case 2: motion_blur_kernel<2><<<grid, 128, 0, s>>>(src, dst, W, H, a); break;
-    case 3: motion_blur_kernel<3><<<grid, 128, 0, s>>>(src, dst, W, H, a); break;
-    case 4:
-      if (((reinterpret_cast<uintptr_t>(src) | reinterpret_cast<uintptr_t>(dst)) & 15) != 0)
-        return fail(MB200_EINVAL, "motion blur: RGBA buffers must be 16-byte aligned");
-      motion_blur_kernel<4><<<grid, 128, 0, s>>>(src, dst, W, H, a);
-      break;
-    default: return fail(MB200_EINVAL, "motion blur: 1..4 channels");
-  }
-  count_launch();
-  const cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return cuda_fail(e, "motion blur launch");
-  return MB200_OK;
+  if (channels == 4 && !aligned16(src, dst)) return fail(MB200_EINVAL, "motion blur: RGBA buffers must be 16-byte aligned");
+  return with_channels(channels, "motion blur", [&](auto ch) {
+    motion_blur_kernel<ch()><<<grid, 128, 0, s>>>(src, dst, W, H, a);
+    return launch_status("motion blur launch");
+  });
 }
 
 int launch_sample(const float *src, size_t w, size_t h, int channels, float *dst, size_t ow, size_t oh, void *stream) {
@@ -289,21 +279,11 @@ int launch_sample(const float *src, size_t w, size_t h, int channels, float *dst
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   dim3 grid(static_cast<unsigned>((ow + 255) / 256), static_cast<unsigned>(oh));
   const int W = static_cast<int>(w), H = static_cast<int>(h), OW = static_cast<int>(ow), OH = static_cast<int>(oh);
-  switch (channels) {
-    case 1: sample_kernel<1><<<grid, 256, 0, s>>>(src, dst, W, H, OW, OH); break;
-    case 2: sample_kernel<2><<<grid, 256, 0, s>>>(src, dst, W, H, OW, OH); break;
-    case 3: sample_kernel<3><<<grid, 256, 0, s>>>(src, dst, W, H, OW, OH); break;
-    case 4:
-      if (((reinterpret_cast<uintptr_t>(src) | reinterpret_cast<uintptr_t>(dst)) & 15) != 0)
-        return fail(MB200_EINVAL, "sample: RGBA buffers must be 16-byte aligned");
-      sample_kernel<4><<<grid, 256, 0, s>>>(src, dst, W, H, OW, OH);
-      break;
-    default: return fail(MB200_EINVAL, "sample: 1..4 channels");
-  }
-  count_launch();
-  const cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return cuda_fail(e, "sample launch");
-  return MB200_OK;
+  if (channels == 4 && !aligned16(src, dst)) return fail(MB200_EINVAL, "sample: RGBA buffers must be 16-byte aligned");
+  return with_channels(channels, "sample", [&](auto ch) {
+    sample_kernel<ch()><<<grid, 256, 0, s>>>(src, dst, W, H, OW, OH);
+    return launch_status("sample launch");
+  });
 }
 
 template <int OP>
@@ -313,21 +293,11 @@ int launch_composite(float *canvas, const float *source, size_t npixels, int cha
   const size_t blocks = (npixels + 255) / 256;
   if (blocks > 0x7fffffffull) return fail(MB200_EINVAL, "composite: image too large");
   const unsigned grid = static_cast<unsigned>(blocks);
-  switch (channels) {
-    case 1: difference_kernel<1, OP><<<grid, 256, 0, s>>>(canvas, source, npixels); break;
-    case 2: difference_kernel<2, OP><<<grid, 256, 0, s>>>(canvas, source, npixels); break;
-    case 3: difference_kernel<3, OP><<<grid, 256, 0, s>>>(canvas, source, npixels); break;
-    case 4:
-      if (((reinterpret_cast<uintptr_t>(canvas) | reinterpret_cast<uintptr_t>(source)) & 15) != 0)
-        return fail(MB200_EINVAL, "composite: RGBA buffers must be 16-byte aligned");
-      difference_kernel<4, OP><<<grid, 256, 0, s>>>(canvas, source, npixels);
-      break;
-    default: return fail(MB200_EINVAL, "composite: 1..4 channels");
-  }
-  count_launch();
-  const cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return cuda_fail(e, "composite launch");
-  return MB200_OK;
+  if (channels == 4 && !aligned16(canvas, source)) return fail(MB200_EINVAL, "composite: RGBA buffers must be 16-byte aligned");
+  return with_channels(channels, "composite", [&](auto ch) {
+    difference_kernel<ch(), OP><<<grid, 256, 0, s>>>(canvas, source, npixels);
+    return launch_status("composite launch");
+  });
 }
 
 int launch_composite_difference(float *canvas, const float *source, size_t npixels, int channels, void *stream) {
@@ -349,21 +319,11 @@ int launch_threshold(float *buf, size_t npixels, int channels, int op, const dou
   const size_t blocks = (npixels + 255) / 256;
   if (blocks > 0x7fffffffull) return fail(MB200_EINVAL, "threshold: image too large");
   const unsigned grid = static_cast<unsigned>(blocks);
-  const bool aligned = (reinterpret_cast<uintptr_t>(buf) & 15) == 0;
-  switch (channels) {
-    case 1: threshold_kernel<1><<<grid, 256, 0, s>>>(buf, npixels, a); break;
-    case 2: threshold_kernel<2><<<grid, 256, 0, s>>>(buf, npixels, a); break;
-    case 3: threshold_kernel<3><<<grid, 256, 0, s>>>(buf, npixels, a); break;
-    case 4:
-      if (!aligned) return fail(MB200_EINVAL, "threshold: RGBA buffers must be 16-byte aligned");
-      threshold_kernel<4><<<grid, 256, 0, s>>>(buf, npixels, a);
-      break;
-    default: return fail(MB200_EINVAL, "threshold: 1..4 channels");
-  }
-  count_launch();
-  const cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return cuda_fail(e, "threshold launch");
-  return MB200_OK;
+  if (channels == 4 && !aligned16(buf)) return fail(MB200_EINVAL, "threshold: RGBA buffers must be 16-byte aligned");
+  return with_channels(channels, "threshold", [&](auto ch) {
+    threshold_kernel<ch()><<<grid, 256, 0, s>>>(buf, npixels, a);
+    return launch_status("threshold launch");
+  });
 }
 
 // Channels outside a `-channel` selection carry the Copy trait: every operator of the path hands them through from its
@@ -396,19 +356,13 @@ __global__ void __launch_bounds__(256) resize_copy_channels_kernel(float *__rest
 
 int launch_restore_channels(float *dst, const float *src, size_t npixels, int channels, unsigned update_mask, void *stream) {
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  const size_t blocks = (npixels + 255) / 256;
-  if (blocks == 0 || blocks > 0x7fffffffull) return fail(MB200_EINVAL, "restore channels: bad image size");
-  const unsigned grid = static_cast<unsigned>(blocks);
-  switch (channels) {
-    case 1: restore_channels_kernel<1><<<grid, 256, 0, s>>>(dst, src, npixels, update_mask); break;
-    case 2: restore_channels_kernel<2><<<grid, 256, 0, s>>>(dst, src, npixels, update_mask); break;
-    case 3: restore_channels_kernel<3><<<grid, 256, 0, s>>>(dst, src, npixels, update_mask); break;
-    case 4: restore_channels_kernel<4><<<grid, 256, 0, s>>>(dst, src, npixels, update_mask); break;
-    default: return fail(MB200_EINVAL, "restore channels: 1..4 channels");
-  }
-  count_launch();
-  const cudaError_t e = cudaGetLastError();
-  return e == cudaSuccess ? MB200_OK : cuda_fail(e, "restore channels launch");
+  unsigned grid;
+  const int rc = grid_of(npixels, 256, &grid, "restore channels");
+  if (rc) return rc;
+  return with_channels(channels, "restore channels", [&](auto ch) {
+    restore_channels_kernel<ch()><<<grid, 256, 0, s>>>(dst, src, npixels, update_mask);
+    return launch_status("restore channels launch");
+  });
 }
 
 int launch_resize_copy_channels(float *dst, const float *src, size_t w, size_t ow, size_t oh, int channels, const int *d_nearest_x,
@@ -417,16 +371,10 @@ int launch_resize_copy_channels(float *dst, const float *src, size_t w, size_t o
   if (oh > 65535) return fail(MB200_EUNSUPPORTED, "resize copy channels: more than 65535 output rows");
   dim3 grid(static_cast<unsigned>((ow + 255) / 256), static_cast<unsigned>(oh));
   const int W = static_cast<int>(w), OW = static_cast<int>(ow), OH = static_cast<int>(oh);
-  switch (channels) {
-    case 1: resize_copy_channels_kernel<1><<<grid, 256, 0, s>>>(dst, src, W, OW, OH, d_nearest_x, d_nearest_y, update_mask); break;
-    case 2: resize_copy_channels_kernel<2><<<grid, 256, 0, s>>>(dst, src, W, OW, OH, d_nearest_x, d_nearest_y, update_mask); break;
-    case 3: resize_copy_channels_kernel<3><<<grid, 256, 0, s>>>(dst, src, W, OW, OH, d_nearest_x, d_nearest_y, update_mask); break;
-    case 4: resize_copy_channels_kernel<4><<<grid, 256, 0, s>>>(dst, src, W, OW, OH, d_nearest_x, d_nearest_y, update_mask); break;
-    default: return fail(MB200_EINVAL, "resize copy channels: 1..4 channels");
-  }
-  count_launch();
-  const cudaError_t e = cudaGetLastError();
-  return e == cudaSuccess ? MB200_OK : cuda_fail(e, "resize copy channels launch");
+  return with_channels(channels, "resize copy channels", [&](auto ch) {
+    resize_copy_channels_kernel<ch()><<<grid, 256, 0, s>>>(dst, src, W, OW, OH, d_nearest_x, d_nearest_y, update_mask);
+    return launch_status("resize copy channels launch");
+  });
 }
 
 // ScaleImage (resize.c:4106): thread = output pixel; out = fold over its column list of (fold over its row list of the
@@ -501,43 +449,34 @@ int launch_scale(const float *src, size_t w, size_t h, int channels, float *dst,
                  const int *d_xidx, const double *d_xwt, const int *d_yoff, const int *d_yidx, const double *d_ywt, void *stream) {
   if (w > 0x3fffffffull || h > 0x3fffffffull || ow > 0x3fffffffull) return fail(MB200_EINVAL, "scale: image too large");
   if (oh > 65535) return fail(MB200_EUNSUPPORTED, "scale: more than 65535 output rows");
-  if (channels == 4 && ((reinterpret_cast<uintptr_t>(src) | reinterpret_cast<uintptr_t>(dst)) & 15) != 0)
-    return fail(MB200_EINVAL, "scale: RGBA buffers must be 16-byte aligned");
+  if (channels == 4 && !aligned16(src, dst)) return fail(MB200_EINVAL, "scale: RGBA buffers must be 16-byte aligned");
   ScaleArgs a{src, dst, static_cast<int>(w), static_cast<int>(h), static_cast<int>(ow), static_cast<int>(oh),
               d_xoff, d_xidx, d_yoff, d_yidx, d_xwt, d_ywt};
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   dim3 grid(static_cast<unsigned>((ow + 127) / 128), static_cast<unsigned>(oh));
-  switch (channels) {
-    case 1: scale_kernel<1><<<grid, 128, 0, s>>>(a); break;
-    case 2: scale_kernel<2><<<grid, 128, 0, s>>>(a); break;
-    case 3: scale_kernel<3><<<grid, 128, 0, s>>>(a); break;
-    case 4: scale_kernel<4><<<grid, 128, 0, s>>>(a); break;
-    default: return fail(MB200_EINVAL, "scale: 1..4 channels");
-  }
-  count_launch();
-  const cudaError_t e = cudaGetLastError();
-  return e == cudaSuccess ? MB200_OK : cuda_fail(e, "scale launch");
+  return with_channels(channels, "scale", [&](auto ch) {
+    scale_kernel<ch()><<<grid, 128, 0, s>>>(a);
+    return launch_status("scale launch");
+  });
 }
 
 int launch_unsharp_combine(const float *src, float *blur_inout, size_t n, double gain, double quantum_threshold,
                            void *stream) {
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  const bool aligned = ((reinterpret_cast<uintptr_t>(src) | reinterpret_cast<uintptr_t>(blur_inout)) & 15) == 0;
-  const size_t n4 = aligned ? n / 4 : 0;
+  const size_t n4 = aligned16(src, blur_inout) ? n / 4 : 0;
+  unsigned launches = 0;
   if (n4) {
     unsharp_kernel<<<static_cast<unsigned>((n4 + 255) / 256), 256, 0, s>>>(
         reinterpret_cast<const float4 *>(src), reinterpret_cast<float4 *>(blur_inout), n4, gain, quantum_threshold);
-    count_launch();
+    ++launches;
   }
   if (n4 * 4 < n) {
     const size_t rest = n - n4 * 4;
     unsharp_tail_kernel<<<static_cast<unsigned>((rest + 255) / 256), 256, 0, s>>>(src, blur_inout, n4 * 4, n, gain,
                                                                                  quantum_threshold);
-    count_launch();
+    ++launches;
   }
-  const cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return cuda_fail(e, "unsharp launch");
-  return MB200_OK;
+  return launch_status("unsharp launch", launches);
 }
 
 }  // namespace mb200

@@ -18,7 +18,7 @@
 //  axis 0 (horizontal): lanes span consecutive OUTPUT columns; weights are stored
 //    tap-major ([tap][o]) so their loads are coalesced; source reads of neighbouring
 //    lanes fall in the same / adjacent 128-byte lines.
-#include "mb200_internal.h"
+#include "launch.cuh"
 
 #include <cuda_runtime.h>
 
@@ -382,45 +382,23 @@ int launch_resize_axis(const float *src, size_t width, size_t height, int channe
   a.o_begin = 0;
   a.o_end = a.out_n;
   if (regular && t.d_wreg != nullptr) {
-    int rc = MB200_EUNSUPPORTED;
-    switch (channels) {
-      case 1: rc = launch_regular_ch<1>(a, axis, t.reg_stride, t.reg_taps, t.d_wreg, t.max_span, s); break;
-      case 2: rc = launch_regular_ch<2>(a, axis, t.reg_stride, t.reg_taps, t.d_wreg, t.max_span, s); break;
-      case 3: rc = launch_regular_ch<3>(a, axis, t.reg_stride, t.reg_taps, t.d_wreg, t.max_span, s); break;
-      default: rc = launch_regular_ch<4>(a, axis, t.reg_stride, t.reg_taps, t.d_wreg, t.max_span, s); break;
-    }
+    const int rc = with_channels(channels, "resize", [&](auto ch) {
+      return launch_regular_ch<ch()>(a, axis, t.reg_stride, t.reg_taps, t.d_wreg, t.max_span, s);
+    });
     if (rc == MB200_OK) {
-      count_launch();
       count_family(kResizeRegular);
-      const cudaError_t e = cudaGetLastError();
-      if (e != cudaSuccess) return cuda_fail(e, "resize launch");
-      return MB200_OK;
+      return launch_status("resize launch");
     }
   }
-  if (axis == 1) {
-    dim3 grid((a.width + 127) / 128, (a.out_n + a.lines_per_thread - 1) / a.lines_per_thread);
-    if (grid.y > 65535) return fail(MB200_EINVAL, "resize: too many rows");
-    switch (channels) {
-      case 1: resize_vertical_kernel<1><<<grid, 128, 0, s>>>(a); break;
-      case 2: resize_vertical_kernel<2><<<grid, 128, 0, s>>>(a); break;
-      case 3: resize_vertical_kernel<3><<<grid, 128, 0, s>>>(a); break;
-      default: resize_vertical_kernel<4><<<grid, 128, 0, s>>>(a); break;
-    }
-  } else {
-    dim3 grid((a.out_n + 127) / 128, (a.height + a.lines_per_thread - 1) / a.lines_per_thread);
-    if (grid.y > 65535) return fail(MB200_EINVAL, "resize: too many rows");
-    switch (channels) {
-      case 1: resize_horizontal_kernel<1><<<grid, 128, 0, s>>>(a); break;
-      case 2: resize_horizontal_kernel<2><<<grid, 128, 0, s>>>(a); break;
-      case 3: resize_horizontal_kernel<3><<<grid, 128, 0, s>>>(a); break;
-      default: resize_horizontal_kernel<4><<<grid, 128, 0, s>>>(a); break;
-    }
-  }
-  count_launch();
-  count_family(kResizeGather);
-  const cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return cuda_fail(e, "resize launch");
-  return MB200_OK;
+  const dim3 grid = axis == 1 ? dim3((a.width + 127) / 128, (a.out_n + a.lines_per_thread - 1) / a.lines_per_thread)
+                              : dim3((a.out_n + 127) / 128, (a.height + a.lines_per_thread - 1) / a.lines_per_thread);
+  if (grid.y > 65535) return fail(MB200_EINVAL, "resize: too many rows");
+  return with_channels(channels, "resize", [&](auto ch) {
+    if (axis == 1) resize_vertical_kernel<ch()><<<grid, 128, 0, s>>>(a);
+    else resize_horizontal_kernel<ch()><<<grid, 128, 0, s>>>(a);
+    count_family(kResizeGather);
+    return launch_status("resize launch");
+  });
 }
 
 }  // namespace mb200

@@ -28,7 +28,7 @@
 //
 // Outputs outside the streamed runs (the image borders, where the window is clipped, and the very
 // short low-binade runs) are produced by the generic gather kernels of resize.cu.
-#include "mb200_internal.h"
+#include "launch.cuh"
 
 #include "tma.cuh"
 
@@ -671,9 +671,7 @@ int launch_resize_fused(const float *src, size_t width, size_t height, float *ds
     resize_border2d_kernel<<<dim3(static_cast<unsigned>((work + 127) / 128), 2), 128, 0, s>>>(b, y.d_is_border);
     count_launch();
   }
-  const cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return cuda_fail(e, "fused resize launch");
-  return MB200_OK;
+  return launch_status("fused resize launch", 0);
 }
 
 namespace {
@@ -771,10 +769,7 @@ int launch_resize_stream(const float *src, size_t width, size_t height, float *d
   else if (stride == 4 && taps == 24) rc = launch_sn<4, 24>(a, axis, s);   // 3-lobe, 4x
   else if (stride == 4 && taps == 16) rc = launch_sn<4, 16>(a, axis, s);   // 2-lobe / cubic, 4x
   if (rc != MB200_OK) return rc;
-  count_launch();
-  const cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return cuda_fail(e, "resize stream launch");
-  return MB200_OK;
+  return launch_status("resize stream launch");
 }
 
 }  // namespace mb200

@@ -10,7 +10,7 @@
 // operation, so the results are bit-identical to the reference's).  Neighbours are fetched through the read-only path
 // (float4 for RGBA); the windows of adjacent threads overlap almost completely, so L1 / L2 serve the re-reads.  These
 // are first, untuned versions (correctness first; DESIGN.md lists their measured throughput).
-#include "mb200_internal.h"
+#include "launch.cuh"
 
 #include <cuda_runtime.h>
 
@@ -526,17 +526,7 @@ int check_image(const float *src, float *dst, size_t w, size_t h, int channels, 
   if (!src || !dst || w == 0 || h == 0 || w > 0x3fffffffull || h > 65535ull * 32768ull) return fail(MB200_EINVAL, "%s: bad geometry", what);
   if (h > 65535) return fail(MB200_EUNSUPPORTED, "%s: more than 65535 rows", what);
   if (channels < 1 || channels > 4) return fail(MB200_EINVAL, "%s: 1..4 channels", what);
-  if (channels == 4 && ((reinterpret_cast<uintptr_t>(src) | reinterpret_cast<uintptr_t>(dst)) & 15) != 0)
-    return fail(MB200_EINVAL, "%s: RGBA buffers must be 16-byte aligned", what);
-  return MB200_OK;
-}
-
-int upload_table(const std::vector<double> &host, double **dev, cudaStream_t s) {
-  cudaError_t e = cudaMallocAsync(reinterpret_cast<void **>(dev), host.size() * sizeof(double), temp_pool(), s);
-  if (e != cudaSuccess) { *dev = nullptr; return cuda_fail(e, "table allocation"); }
-  // pageable source: the runtime stages it before returning, so `host` may die right after the call
-  e = cudaMemcpyAsync(*dev, host.data(), host.size() * sizeof(double), cudaMemcpyHostToDevice, s);
-  if (e != cudaSuccess) { cudaFreeAsync(*dev, s); *dev = nullptr; return cuda_fail(e, "table upload"); }
+  if (channels == 4 && !aligned16(src, dst)) return fail(MB200_EINVAL, "%s: RGBA buffers must be 16-byte aligned", what);
   return MB200_OK;
 }
 
@@ -552,15 +542,10 @@ int launch_statistic(const float *src, float *dst, size_t w, size_t h, int chann
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   dim3 grid(static_cast<unsigned>((w + 127) / 128), static_cast<unsigned>(h));
   const int iw = static_cast<int>(w), ih = static_cast<int>(h), iW = static_cast<int>(W), iH = static_cast<int>(H);
-  switch (channels) {
-    case 1: statistic_kernel<1><<<grid, 128, 0, s>>>(src, dst, iw, ih, type, iW, iH); break;
-    case 2: statistic_kernel<2><<<grid, 128, 0, s>>>(src, dst, iw, ih, type, iW, iH); break;
-    case 3: statistic_kernel<3><<<grid, 128, 0, s>>>(src, dst, iw, ih, type, iW, iH); break;
-    default: statistic_kernel<4><<<grid, 128, 0, s>>>(src, dst, iw, ih, type, iW, iH); break;
-  }
-  count_launch();
-  const cudaError_t e = cudaGetLastError();
-  return e == cudaSuccess ? MB200_OK : cuda_fail(e, "statistic launch");
+  return with_channels(channels, "statistic", [&](auto ch) {
+    statistic_kernel<ch()><<<grid, 128, 0, s>>>(src, dst, iw, ih, type, iW, iH);
+    return launch_status("statistic launch");
+  });
 }
 
 int launch_rotational_blur(const float *src, float *dst, size_t w, size_t h, int channels, double angle, void *stream) {
@@ -580,21 +565,15 @@ int launch_rotational_blur(const float *src, float *dst, size_t w, size_t h, int
     tables[n + k] = std::sin(theta * static_cast<double>(static_cast<long>(k)) - offset);
   }
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  double *d_tables = nullptr;
-  rc = upload_table(tables, &d_tables, s);
-  if (rc) return rc;
+  StreamAlloc table(s);
+  if ((rc = table.upload(tables.data(), tables.size() * sizeof(double), "rotational blur: table upload"))) return rc;
+  const double *d_tables = table.as<double>();
   dim3 grid(static_cast<unsigned>((w + 127) / 128), static_cast<unsigned>(h));
   const int iw = static_cast<int>(w), ih = static_cast<int>(h), in = static_cast<int>(n);
-  switch (channels) {
-    case 1: rotational_blur_kernel<1><<<grid, 128, 0, s>>>(src, dst, iw, ih, d_tables, d_tables + n, in, cx, cy, blur_radius); break;
-    case 2: rotational_blur_kernel<2><<<grid, 128, 0, s>>>(src, dst, iw, ih, d_tables, d_tables + n, in, cx, cy, blur_radius); break;
-    case 3: rotational_blur_kernel<3><<<grid, 128, 0, s>>>(src, dst, iw, ih, d_tables, d_tables + n, in, cx, cy, blur_radius); break;
-    default: rotational_blur_kernel<4><<<grid, 128, 0, s>>>(src, dst, iw, ih, d_tables, d_tables + n, in, cx, cy, blur_radius); break;
-  }
-  count_launch();
-  const cudaError_t e = cudaGetLastError();
-  cudaFreeAsync(d_tables, s);
-  return e == cudaSuccess ? MB200_OK : cuda_fail(e, "rotational blur launch");
+  return with_channels(channels, "rotational blur", [&](auto ch) {
+    rotational_blur_kernel<ch()><<<grid, 128, 0, s>>>(src, dst, iw, ih, d_tables, d_tables + n, in, cx, cy, blur_radius);
+    return launch_status("rotational blur launch");
+  });
 }
 
 int launch_bilateral_blur(const float *src, float *dst, size_t w, size_t h, int channels, size_t width, size_t height,
@@ -622,31 +601,20 @@ int launch_bilateral_blur(const float *src, float *dst, size_t w, size_t h, int 
       tables[n++] = blur_gaussian(std::sqrt(dx * dx + dy * dy), spatial_sigma);
     }
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  double *d_tables = nullptr;
-  unsigned char *d_i8 = nullptr;
-  rc = upload_table(tables, &d_tables, s);
-  if (rc) return rc;
-  cudaError_t e = cudaMallocAsync(reinterpret_cast<void **>(&d_i8), w * h, temp_pool(), s);
-  if (e != cudaSuccess) { cudaFreeAsync(d_tables, s); return cuda_fail(e, "bilateral blur: intensity plane"); }
+  StreamAlloc table(s), plane(s);
+  if ((rc = table.upload(tables.data(), tables.size() * sizeof(double), "bilateral blur: table upload"))) return rc;
+  if ((rc = plane.alloc(w * h, "bilateral blur: intensity plane"))) return rc;
+  const double *d_tables = table.as<double>();
+  unsigned char *d_i8 = plane.as<unsigned char>();
   const size_t npix = w * h;
   const unsigned pgrid = static_cast<unsigned>((npix + 255) / 256);
   dim3 grid(static_cast<unsigned>((w + 127) / 128), static_cast<unsigned>(h));
   const int iw = static_cast<int>(w), ih = static_cast<int>(h), iW = static_cast<int>(W), iH = static_cast<int>(H);
-  switch (channels) {
-    case 1: intensity8_kernel<1><<<pgrid, 256, 0, s>>>(src, d_i8, npix);
-            bilateral_kernel<1><<<grid, 128, 0, s>>>(src, d_i8, dst, iw, ih, iW, iH, d_tables, d_tables + 512); break;
-    case 2: intensity8_kernel<2><<<pgrid, 256, 0, s>>>(src, d_i8, npix);
-            bilateral_kernel<2><<<grid, 128, 0, s>>>(src, d_i8, dst, iw, ih, iW, iH, d_tables, d_tables + 512); break;
-    case 3: intensity8_kernel<3><<<pgrid, 256, 0, s>>>(src, d_i8, npix);
-            bilateral_kernel<3><<<grid, 128, 0, s>>>(src, d_i8, dst, iw, ih, iW, iH, d_tables, d_tables + 512); break;
-    default: intensity8_kernel<4><<<pgrid, 256, 0, s>>>(src, d_i8, npix);
-             bilateral_kernel<4><<<grid, 128, 0, s>>>(src, d_i8, dst, iw, ih, iW, iH, d_tables, d_tables + 512); break;
-  }
-  count_launch(2);
-  e = cudaGetLastError();
-  cudaFreeAsync(d_i8, s);
-  cudaFreeAsync(d_tables, s);
-  return e == cudaSuccess ? MB200_OK : cuda_fail(e, "bilateral blur launch");
+  return with_channels(channels, "bilateral blur", [&](auto ch) {
+    intensity8_kernel<ch()><<<pgrid, 256, 0, s>>>(src, d_i8, npix);
+    bilateral_kernel<ch()><<<grid, 128, 0, s>>>(src, d_i8, dst, iw, ih, iW, iH, d_tables, d_tables + 512);
+    return launch_status("bilateral blur launch", 2);
+  });
 }
 
 int launch_selective_blur(const float *src, float *dst, size_t w, size_t h, int channels, double radius, double sigma,
@@ -665,39 +633,23 @@ int launch_selective_blur(const float *src, float *dst, size_t w, size_t h, int 
     for (long u = -j; u <= j; ++u)
       taps[n++] = std::exp(-(static_cast<double>(u) * u + v * v) / (2.0 * sg * sg)) / (2.0 * kPi * sg * sg);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  double *d_taps = nullptr, *d_lum = nullptr;
-  rc = upload_table(taps, &d_taps, s);
-  if (rc) return rc;
   const size_t npix = w * h;
-  cudaError_t e = cudaMallocAsync(reinterpret_cast<void **>(&d_lum), npix * sizeof(double), temp_pool(), s);
-  if (e != cudaSuccess) { cudaFreeAsync(d_taps, s); return cuda_fail(e, "selective blur: intensity plane"); }
+  StreamAlloc table(s), plane(s);
+  if ((rc = table.upload(taps.data(), taps.size() * sizeof(double), "selective blur: table upload"))) return rc;
+  if ((rc = plane.alloc(npix * sizeof(double), "selective blur: intensity plane"))) return rc;
+  const double *d_taps = table.as<double>();
+  double *d_lum = plane.as<double>();
   const unsigned pgrid = static_cast<unsigned>((npix + 255) / 256);
   dim3 grid(static_cast<unsigned>((w + 127) / 128), static_cast<unsigned>(h));
   const int iw = static_cast<int>(w), ih = static_cast<int>(h), iW = static_cast<int>(W);
-  switch (channels) {
-    case 1: intensity_plane_kernel<1><<<pgrid, 256, 0, s>>>(src, d_lum, npix);
-            selective_blur_kernel<1><<<grid, 128, 0, s>>>(src, d_lum, dst, iw, ih, iW, d_taps, threshold); break;
-    case 2: intensity_plane_kernel<2><<<pgrid, 256, 0, s>>>(src, d_lum, npix);
-            selective_blur_kernel<2><<<grid, 128, 0, s>>>(src, d_lum, dst, iw, ih, iW, d_taps, threshold); break;
-    case 3: intensity_plane_kernel<3><<<pgrid, 256, 0, s>>>(src, d_lum, npix);
-            selective_blur_kernel<3><<<grid, 128, 0, s>>>(src, d_lum, dst, iw, ih, iW, d_taps, threshold); break;
-    default: intensity_plane_kernel<4><<<pgrid, 256, 0, s>>>(src, d_lum, npix);
-             selective_blur_kernel<4><<<grid, 128, 0, s>>>(src, d_lum, dst, iw, ih, iW, d_taps, threshold); break;
-  }
-  count_launch(2);
-  e = cudaGetLastError();
-  cudaFreeAsync(d_lum, s);
-  cudaFreeAsync(d_taps, s);
-  return e == cudaSuccess ? MB200_OK : cuda_fail(e, "selective blur launch");
+  return with_channels(channels, "selective blur", [&](auto ch) {
+    intensity_plane_kernel<ch()><<<pgrid, 256, 0, s>>>(src, d_lum, npix);
+    selective_blur_kernel<ch()><<<grid, 128, 0, s>>>(src, d_lum, dst, iw, ih, iW, d_taps, threshold);
+    return launch_status("selective blur launch", 2);
+  });
 }
 
 namespace {
-
-template <int CH>
-void launch_exact(const float *src, float *dst, int w, int h, const double *cells, int kw, int kh, int ox, int oy, cudaStream_t s) {
-  dim3 grid(static_cast<unsigned>((w + 127) / 128), static_cast<unsigned>(h));
-  exact_convolve_kernel<CH><<<grid, 128, 0, s>>>(src, dst, w, h, cells, kw, kh, ox, oy);
-}
 
 // one ConvolveMorphology stage with the kernel's cells reflected on the host (morphology.c:2612-2626)
 int exact_convolve(const float *src, float *dst, size_t w, size_t h, int channels, const mb200_kernel_info *k, cudaStream_t s) {
@@ -707,21 +659,16 @@ int exact_convolve(const float *src, float *dst, size_t w, size_t h, int channel
     if (k->values[i] != k->values[i]) return fail(MB200_EUNSUPPORTED, "adaptive: kernel with NaN cells");
     cells[i] = k->values[n - 1 - i];
   }
-  double *d_cells = nullptr;
-  int rc = upload_table(cells, &d_cells, s);
+  StreamAlloc table(s);
+  const int rc = table.upload(cells.data(), cells.size() * sizeof(double), "adaptive: table upload");
   if (rc) return rc;
   const int iw = static_cast<int>(w), ih = static_cast<int>(h), kw = static_cast<int>(k->width), kh = static_cast<int>(k->height);
   const int ox = kw - static_cast<int>(k->x) - 1, oy = kh - static_cast<int>(k->y) - 1;
-  switch (channels) {
-    case 1: launch_exact<1>(src, dst, iw, ih, d_cells, kw, kh, ox, oy, s); break;
-    case 2: launch_exact<2>(src, dst, iw, ih, d_cells, kw, kh, ox, oy, s); break;
-    case 3: launch_exact<3>(src, dst, iw, ih, d_cells, kw, kh, ox, oy, s); break;
-    default: launch_exact<4>(src, dst, iw, ih, d_cells, kw, kh, ox, oy, s); break;
-  }
-  count_launch();
-  const cudaError_t e = cudaGetLastError();
-  cudaFreeAsync(d_cells, s);
-  return e == cudaSuccess ? MB200_OK : cuda_fail(e, "adaptive: convolution launch");
+  const dim3 grid(static_cast<unsigned>((iw + 127) / 128), static_cast<unsigned>(ih));
+  return with_channels(channels, "adaptive", [&](auto ch) {
+    exact_convolve_kernel<ch()><<<grid, 128, 0, s>>>(src, dst, iw, ih, table.as<const double>(), kw, kh, ox, oy);
+    return launch_status("adaptive: convolution launch");
+  });
 }
 
 // AutoLevelImage with the default channel mask (enhance.c:266 -> histogram.c:942-953): level.cu's MinMaxStretchImage,
@@ -729,18 +676,6 @@ int exact_convolve(const float *src, float *dst, size_t w, size_t h, int channel
 int auto_level(float *buf, size_t w, size_t h, int channels, cudaStream_t s) {
   return launch_minmax_stretch(buf, w, h, channels, 0.0, 0.0, 1.0, false, (1u << channels) - 1u, s);
 }
-
-struct DeviceTemp {
-  void *p = nullptr;
-  cudaStream_t s;
-  explicit DeviceTemp(cudaStream_t stream) : s(stream) {}
-  ~DeviceTemp() { if (p) cudaFreeAsync(p, s); }
-  int alloc(size_t bytes) {
-    const cudaError_t e = cudaMallocAsync(&p, bytes ? bytes : 1, temp_pool(), s);
-    if (e != cudaSuccess) { p = nullptr; return cuda_fail(e, "adaptive: temporary"); }
-    return MB200_OK;
-  }
-};
 
 }  // namespace
 
@@ -780,11 +715,10 @@ int launch_adaptive(const float *src, float *dst, size_t w, size_t h, int channe
   const KernelList edge_k(mb200_edge_kernel(radius)), blur_k = blur_kernel_pair(radius, sigma);
   if (!edge_k || !blur_k) return fail(MB200_ENOMEM, "adaptive: kernels");
 
-  DeviceTemp edge(s), tmp(s), d_offsets(s);
-  if ((rc = edge.alloc(n * sizeof(float))) || (rc = tmp.alloc(n * sizeof(float))) ||
-      (rc = d_offsets.alloc(offsets.size() * sizeof(int))))
+  StreamAlloc edge(s), tmp(s), d_offsets(s), d_kernels(s);
+  if ((rc = edge.alloc(n * sizeof(float), "adaptive: temporary")) || (rc = tmp.alloc(n * sizeof(float), "adaptive: temporary")))
     return rc;
-  float *d_edge = static_cast<float *>(edge.p), *d_tmp = static_cast<float *>(tmp.p);
+  float *d_edge = edge.as<float>(), *d_tmp = tmp.as<float>();
   // EdgeImage -> AutoLevel -> BlurImage (row kernel, then the rotated one: float intermediate) -> AutoLevel
   if ((rc = exact_convolve(src, d_edge, w, h, channels, edge_k.get(), s))) return rc;
   if ((rc = auto_level(d_edge, w, h, channels, s))) return rc;
@@ -792,23 +726,16 @@ int launch_adaptive(const float *src, float *dst, size_t w, size_t h, int channe
   if ((rc = exact_convolve(d_tmp, d_edge, w, h, channels, blur_k->next, s))) return rc;
   if ((rc = auto_level(d_edge, w, h, channels, s))) return rc;
 
-  double *d_kernels = nullptr;
-  if ((rc = upload_table(kernels, &d_kernels, s))) return rc;
-  cudaError_t e = cudaMemcpyAsync(d_offsets.p, offsets.data(), offsets.size() * sizeof(int), cudaMemcpyHostToDevice, s);
-  if (e != cudaSuccess) { cudaFreeAsync(d_kernels, s); return cuda_fail(e, "adaptive: offsets upload"); }
+  if ((rc = d_kernels.upload(kernels.data(), kernels.size() * sizeof(double), "adaptive: table upload")) ||
+      (rc = d_offsets.upload(offsets.data(), offsets.size() * sizeof(int), "adaptive: offsets upload")))
+    return rc;
   dim3 grid(static_cast<unsigned>((w + 127) / 128), static_cast<unsigned>(h));
   const int iw = static_cast<int>(w), ih = static_cast<int>(h), iwidth = static_cast<int>(width);
-  const int *d_off = static_cast<const int *>(d_offsets.p);
-  switch (channels) {
-    case 1: adaptive_kernel<1><<<grid, 128, 0, s>>>(src, d_edge, dst, iw, ih, iwidth, d_kernels, d_off); break;
-    case 2: adaptive_kernel<2><<<grid, 128, 0, s>>>(src, d_edge, dst, iw, ih, iwidth, d_kernels, d_off); break;
-    case 3: adaptive_kernel<3><<<grid, 128, 0, s>>>(src, d_edge, dst, iw, ih, iwidth, d_kernels, d_off); break;
-    default: adaptive_kernel<4><<<grid, 128, 0, s>>>(src, d_edge, dst, iw, ih, iwidth, d_kernels, d_off); break;
-  }
-  count_launch();
-  e = cudaGetLastError();
-  cudaFreeAsync(d_kernels, s);
-  return e == cudaSuccess ? MB200_OK : cuda_fail(e, "adaptive: launch");
+  return with_channels(channels, "adaptive", [&](auto ch) {
+    adaptive_kernel<ch()><<<grid, 128, 0, s>>>(src, d_edge, dst, iw, ih, iwidth, d_kernels.as<const double>(),
+                                              d_offsets.as<const int>());
+    return launch_status("adaptive: launch");
+  });
 }
 
 }  // namespace mb200

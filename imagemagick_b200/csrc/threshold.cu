@@ -22,7 +22,7 @@
 //
 // AutoThresholdImage (:660): the threshold of Kapur (:391), OTSU (:491) and Triangle (:570) from the normalised 256-bin
 // histogram, on the host in the reference's order with the same libm calls (auto_threshold_percent).
-#include "mb200_internal.h"
+#include "launch.cuh"
 
 #include <cuda_runtime.h>
 
@@ -194,21 +194,15 @@ int launch_adaptive_ch(const AdaptiveArgs &a, bool tile, size_t smem, cudaStream
     if (e != cudaSuccess) return cuda_fail(e, "adaptive threshold: shared memory attribute");
     adaptive_tile_kernel<CH><<<(a.height + kRows - 1) / kRows, kRows * CH, smem, s>>>(a);
     count_family(kAdaptiveThresholdTile);
-    count_launch();
-    const cudaError_t le = cudaGetLastError();
-    return le == cudaSuccess ? MB200_OK : cuda_fail(le, "adaptive threshold tile launch");
+    return launch_status("adaptive threshold tile launch");
   }
-  double *ring = nullptr;
-  const size_t ring_bytes = sizeof(double) * a.w * static_cast<size_t>(a.height) * CH;
-  cudaError_t e = cudaMallocAsync(reinterpret_cast<void **>(&ring), ring_bytes, temp_pool(), s);
-  if (e != cudaSuccess) return cuda_fail(e, "adaptive threshold: ring allocation");
+  StreamAlloc ring(s);
+  const int rc = ring.alloc(sizeof(double) * a.w * static_cast<size_t>(a.height) * CH, "adaptive threshold: ring allocation");
+  if (rc) return rc;
   const long chains = static_cast<long>(a.height) * CH;
-  adaptive_direct_kernel<CH><<<static_cast<unsigned>((chains + 127) / 128), 128, 0, s>>>(a, ring);
+  adaptive_direct_kernel<CH><<<static_cast<unsigned>((chains + 127) / 128), 128, 0, s>>>(a, ring.as<double>());
   count_family(kAdaptiveThresholdDirect);
-  count_launch();
-  e = cudaGetLastError();
-  cudaFreeAsync(ring, s);
-  return e == cudaSuccess ? MB200_OK : cuda_fail(e, "adaptive threshold direct launch");
+  return launch_status("adaptive threshold direct launch");
 }
 
 }  // namespace
@@ -229,12 +223,7 @@ int launch_adaptive_threshold(const float *src, float *dst, size_t width, size_t
   cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device);
   const size_t smem = tile_bytes(channels, a.w, a.h, &a.pitch);
   const bool tile = smem <= static_cast<size_t>(optin) && !tuning_knobs().no_adaptive_tile;
-  switch (channels) {
-    case 1: return launch_adaptive_ch<1>(a, tile, smem, s);
-    case 2: return launch_adaptive_ch<2>(a, tile, smem, s);
-    case 3: return launch_adaptive_ch<3>(a, tile, smem, s);
-    default: return launch_adaptive_ch<4>(a, tile, smem, s);
-  }
+  return with_channels(channels, "adaptive threshold", [&](auto ch) { return launch_adaptive_ch<ch()>(a, tile, smem, s); });
 }
 
 namespace {
